@@ -30,8 +30,11 @@ import numpy as np  # noqa: E402
 N_TRAIN = 65536
 N_TEST = 4096
 SIGMA2 = 0.1
-DEFAULT_TRAILING = "ozaki"
-DMMA_PEAK_TFLOPS = 37.1  # builder-measured, tools/mb_fp64_peak.cu on this pool's B200 (profiles/)
+DEFAULT_TRAILING = "dmma"
+# NVIDIA H100 SXM data sheet (700 W), dense: the denominators of the roofline fractions, not reached rates
+DMMA_PEAK_TFLOPS = 67.0
+INT8_PEAK_TOPS = 1979.0
+HBM_PEAK_GBS = 3350.0
 
 
 _OUT_FD = None  # set by main(): the process's ORIGINAL stdout; fd 1 itself is pointed at stderr
@@ -298,6 +301,11 @@ def gpu_main(args):
     dev_ms = ctx.elapsed_ms(0, 1)  # CUDA events on the launching (library) stream around K steps
     torch.cuda.synchronize()
     wall_dev = time.perf_counter() - t0
+    if args.dump_outputs and rank == 0:
+        # what a caller of the timed path received in its last step (seeded inputs: comparable across builds)
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, a in (("logpdf", np.array([lp])), ("mean", mean_d.cpu().numpy()), ("var", var_d.cpu().numpy())):
+            np.save(os.path.join(args.dump_outputs, f"{name}.npy"), a.astype(np.float64))
     tm = ctx.timings()
     clocks = sampler.stop() if rank == 0 else None
     step_ms = dev_ms / args.steps
@@ -346,8 +354,8 @@ def gpu_main(args):
     mean_h, var_h = mean_d.cpu().numpy(), var_d.cpu().numpy()
     np.testing.assert_allclose(mean_h, m_e, rtol=1e-9, atol=1e-10)
     # ---- parity against the committed single-GPU result of the same seeded inputs -----------------
-    # (tests/golden/config2_n1.json: written by a 1-GPU DMMA run, itself oracle-checked at N <= 32768
-    #  and cross-checked against the tcgen05 path at full size in tests/test_gpu_parity.py)
+    # (tests/golden/config2_n1.json: written by a 1-GPU run, itself oracle-checked at N <= 32768
+    #  and cross-checked between the DMMA and int8 Ozaki paths at full size in tests/test_gpu_parity.py)
     gold_path = os.path.join(ROOT, "tests", "golden", "config2_n1.json")
     parity = None
     if args.write_golden and args.gpus == 1 and (n, ns) == (N_TRAIN, N_TEST):
@@ -366,27 +374,14 @@ def gpu_main(args):
                             and parity["var_max_rel_err"] <= 1e-8)
 
     # ---- roofline of the dominant kernel (the trailing update of the Cholesky) -----------------------
-    peaks = {}
-    try:
-        peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-        pass
-    traffic = None
-    try:  # per-launch DRAM bytes of the shipped trailing kernel from a committed `ncu --set full` capture
-        traffic = json.load(open(os.path.join(ROOT, "profiles", "roofline_traffic.json"))).get(args.trailing)
-    except Exception:
-        pass
     t_ms = tm["trailing_kernel_ms"]
     fp64_tf = tm["trailing_flops"] / (t_ms * 1e-3) / 1e12 if t_ms else None
     if tm.get("trailing_int8_ops", 0) > 0:
-        # tcgen05 kind::i8: 28 int8 MMAs per fp64 MMA.  Peak = 2 x the MEASURED dense bf16 tensor peak
-        # (int8 runs at twice the bf16 rate on sm_100a); sustained figure: the kernel runs inside a long step.
-        bf16 = peaks.get("bf16_tflops_sustained", 1400.0)
-        peak = 2.0 * bf16
+        # wgmma s8: 28 int8 MMAs per fp64 MMA
         ach = tm["trailing_int8_ops"] / (t_ms * 1e-3) / 1e12
-        roof = {"bound": "tensor", "kernel": "ozaki_syrk_kernel (tcgen05.mma kind::i8 from TMEM, fp64 via 7 int8 digit planes)",
-                "achieved": ach, "peak": peak, "unit": "TOP/s (int8)", "frac": ach / peak,
-                "peak_source": ("2 x MEASURED_PEAKS.json bf16_tflops_sustained" if peaks else "2 x fallback 1400 TF (of fallback)"),
+        roof = {"bound": "tensor", "kernel": "ozaki_syrk_kernel (wgmma s8, fp64 via 7 int8 digit planes)",
+                "achieved": ach, "peak": INT8_PEAK_TOPS, "unit": "TOP/s (int8)", "frac": ach / INT8_PEAK_TOPS,
+                "peak_source": "NVIDIA H100 SXM data sheet, dense int8, 700 W",
                 "fp64_equivalent_tflops": fp64_tf, "vs_dmma_peak": fp64_tf / DMMA_PEAK_TFLOPS if fp64_tf else None,
                 "launches": tm["trailing_launches"] // max(1, args.steps),
                 "flops_per_step": tm["trailing_flops"] / args.steps,
@@ -395,20 +390,13 @@ def gpu_main(args):
         roof = {"bound": "tensor", "kernel": "gemm_nt_kernel (fp64 DMMA SYRK trailing update)",
                 "achieved": fp64_tf, "peak": DMMA_PEAK_TFLOPS, "unit": "TFLOP/s",
                 "frac": (fp64_tf / DMMA_PEAK_TFLOPS) if fp64_tf else None,
-                "peak_source": "builder-measured mma.sync m8n8k4 f64 microbenchmark (tools/mb_fp64_peak.cu, "
-                               "profiles/mb_fp64_peak_r1.txt); MEASURED_PEAKS.json has no fp64 entry, "
-                               "tcgen05 has no fp64 kind",
+                "peak_source": "NVIDIA H100 SXM data sheet, dense fp64 tensor core, 700 W",
                 "launches": tm["trailing_launches"] // max(1, args.steps),
                 "flops_per_step": tm["trailing_flops"] / args.steps}
-    roof["traffic"] = traffic["dram_bytes_per_launch"] if traffic else None
-    if traffic:
-        roof["traffic_algorithmic"] = traffic.get("algorithmic_bytes_per_launch")
-        roof["traffic_source"] = traffic.get("source")
-    hbm_peak = peaks.get("hbm_gbs", 6650.0)
     asm_bytes = (n * (n + 1) / 2 * 8 + n * 8)
     roof_asm = {"bound": "hbm", "kernel": "assemble_kernel<packed>", "achieved": asm_bytes / (tm["assemble_ms"] / args.steps * 1e-3) / 1e9,
-                "peak": hbm_peak, "unit": "GB/s"}
-    roof_asm["frac"] = roof_asm["achieved"] / hbm_peak
+                "peak": HBM_PEAK_GBS, "unit": "GB/s"}
+    roof_asm["frac"] = roof_asm["achieved"] / HBM_PEAK_GBS
     phases = {k: tm[k] / args.steps for k in ("assemble_ms", "panel_ms", "trailing_ms", "comm_ms", "solve_ms", "predict_ms", "panel_chain_ms")}
 
     cb = None
@@ -446,7 +434,7 @@ def reference_main(args):
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
         return
-    reps = max(1, min(args.steps, 3))
+    reps = args.steps
     if args.warmup > 0:
         run_cpu_sample(4096, 1)   # page in NumPy/SciPy/OpenBLAS, spin up the thread pool
     s = run_cpu_sample(reps=reps)
@@ -454,8 +442,8 @@ def reference_main(args):
     val = N_TRAIN / ext
     out = {
         "impl": "reference", "metric": "logpdf+posterior points/sec, N=65536 SE-GP fp64", "value": val,
-        "unit": "points/s", "n_gpus": args.gpus, "steps": reps, "steps_requested": args.steps, "warmup": args.warmup,
-        "samples_run": reps, "ms_per_step": ext * 1e3, "higher_is_better": True, "scaling": "strong", "vs_baseline": None,
+        "unit": "points/s", "n_gpus": args.gpus, "steps": reps, "warmup": args.warmup,
+        "ms_per_step": ext * 1e3, "higher_is_better": True, "scaling": "strong", "vs_baseline": None,
         "dtype": "f64", "data": "synthetic",
         "config": {"workload": f"config 2: SEKernel GP N={N_TRAIN} fp64: kernelmatrix + Cholesky logpdf + "
                                f"posterior mean/var at N*={N_TEST} (CPU restatement of the reference path; "
@@ -484,8 +472,16 @@ def main():
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--write-golden", action="store_true", help="(1 GPU) rewrite tests/golden/config2_n1.json")
     ap.add_argument("--trailing", default=os.environ.get("SB_BENCH_TRAILING", DEFAULT_TRAILING), choices=["dmma", "ozaki"],
-                    help="Cholesky trailing update: fp64 DMMA (mma.sync) or tcgen05 int8 Ozaki slices")
+                    help="Cholesky trailing update: fp64 DMMA (mma.sync) or int8 Ozaki slices (wgmma)")
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="write logpdf, posterior mean and variance of the last timed step as DIR/<name>.npy (float64)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.warmup < 0:
+        ap.error("--warmup must not be negative")
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs writes the outputs of the GPU arm; the reference arm only times a CPU sample")
     global _OUT_FD
     sys.stdout.flush()
     _OUT_FD = os.dup(1)

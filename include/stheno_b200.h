@@ -1,6 +1,6 @@
-/* stheno_b200.h -- C ABI of the B200-native dense-GP hot path (libstheno_b200.so).
+/* stheno_b200.h -- C ABI of the H100-native (sm_90a) dense-GP hot path (libstheno_b200.so).
  *
- * The reference (Stheno.jl, /root/reference) has no FFI: its seam is Julia dispatch on the
+ * The reference (Stheno.jl) has no FFI: its seam is Julia dispatch on the
  * "internal AbstractGPs API" (docs/src/internals.md:8-24) -- AbstractGPs calls
  * mean/cov/var(f, x[, x']) on the GPPP (src/gaussian_process_probabilistic_programme.jl:45-80)
  * and then does cholesky/logdet/solves itself on host matrices.  This ABI intercepts ONE LEVEL
@@ -122,7 +122,7 @@ typedef struct {
 typedef struct {
     double assemble_ms; /* K1 tile assembly */
     double panel_ms;    /* panel work on the critical path: first serial phase + the tensor-core panel solves */
-    double trailing_ms; /* SYRK/GEMM trailing updates (tcgen05 int8 slices, or DMMA) */
+    double trailing_ms; /* SYRK/GEMM trailing updates (DMMA, or int8 Ozaki slices) */
     double solve_ms;    /* vector triangular solves + reductions */
     double predict_ms;  /* cross assembly + matrix TRSM + mean/var */
     double comm_ms;     /* block-column exchange (peer copies; NCCL broadcast on the fallback path), incl. waiting for the owners */
@@ -131,7 +131,7 @@ typedef struct {
     double trailing_kernel_ms; /* sum of per-launch CUDA-event durations of that kernel */
     int64_t trailing_launches;
     int64_t kernel_launches; /* all kernels launched by this library since last reset */
-    double trailing_int8_ops; /* int8 tensor-core ops (2 * MACs) issued by the tcgen05 trailing kernel; 0 on the DMMA path */
+    double trailing_int8_ops; /* int8 tensor-core ops (2 * MACs) issued by the int8 Ozaki trailing kernel; 0 on the DMMA path */
     double panel_chain_ms;    /* total duration of the serial panel phases on the second stream (hidden under T^B) */
 } sb_timings;
 
@@ -151,7 +151,7 @@ int32_t sb_ctx_create_dist(int32_t device, int32_t rank, int32_t world, const vo
                            sb_ctx** out);
 int32_t sb_ctx_destroy(sb_ctx* ctx);
 int32_t sb_ctx_timings(sb_ctx* ctx, sb_timings* out, int32_t reset);
-/* options: "trailing" = 0 fp64 DMMA (mma.sync) | 1 tcgen05 int8 Ozaki slices fed from TMEM (also env
+/* options: "trailing" = 0 fp64 DMMA (mma.sync, default) | 1 int8 Ozaki slices on wgmma (also env
  * SB_TRAILING=dmma|ozaki at context creation); "fine_timing" = 0 | 1. */
 int32_t sb_ctx_set_option(sb_ctx* ctx, const char* key, int64_t value);
 /* benchmark support: record a CUDA event on the library's stream into slot 0..7 / read the

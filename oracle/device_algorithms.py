@@ -1,7 +1,7 @@
 """CPU RESTATEMENT OF THE DEVICE-SIDE NUMERICAL SCHEMES -- TEST INFRASTRUCTURE ONLY.  NOT A PRODUCT PATH.
 
 Nothing here follows a reference file: the reference (Stheno.jl) calls LAPACK `dpotrf` / `dtrsm`
-(SURVEY.md App. A) and has no counterpart for *how* the B200 library reaches the same numbers.  These are
+(SURVEY.md App. A) and has no counterpart for *how* the CUDA library reaches the same numbers.  These are
 plain NumPy statements of three device algorithms, so that their mathematics is pinned on the CPU against
 LAPACK / exact arithmetic and the CUDA sources can cite a runnable specification:
 

@@ -1,7 +1,7 @@
 """CPU ORACLE -- TEST INFRASTRUCTURE ONLY.  NOT A PRODUCT PATH.
 
 A NumPy/SciPy(OpenBLAS) restatement of the reference algorithm for the dense-GP hot path
-of Stheno.jl (reference @ /root/reference, commit 905f995, v0.8.2).  Only `tests/`,
+of Stheno.jl (commit 905f995, v0.8.2).  Only `tests/`,
 `__graft_entry__.smoke()` and `bench.py`'s cpu_baseline / `--impl reference` leg may import
 this module, and only as the checker / reported baseline.
 

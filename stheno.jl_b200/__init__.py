@@ -1,4 +1,4 @@
-"""stheno.jl_b200 -- B200-native dense-GP inference hot path behind the Stheno/AbstractGPs API.
+"""stheno.jl_b200 -- H100-native dense-GP inference hot path behind the Stheno/AbstractGPs API.
 
 Only what the path needs: `csrc/` (CUDA kernels + C ABI -> libstheno_b200.so), `lib.py` (ctypes
 binding == what the Julia shim `ccall`s), `inputs.py` / `gp.py` / `finite.py` (host-side mirror

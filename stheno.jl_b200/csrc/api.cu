@@ -30,10 +30,7 @@ int32_t cuda_fail(cudaError_t e, const char* what, const char* file, int line) {
 using namespace sb;
 
 #ifndef SB_DEFAULT_TRAILING
-#define SB_DEFAULT_TRAILING 1   /* tcgen05 int8 Ozaki trailing update (SB_TRAILING=dmma selects the fp64 DMMA path) */
-#endif
-#ifndef SB_DEFAULT_OZ_MODE
-#define SB_DEFAULT_OZ_MODE 8   /* SWIZZLE_64B operands, 2 x 84 KB stages, paired N=128 MMAs (fastest measured) */
+#define SB_DEFAULT_TRAILING 0   /* fp64 DMMA trailing update, the faster path on H100 (SB_TRAILING=ozaki selects int8 Ozaki) */
 #endif
 
 // NCCL is bound lazily with dlopen (only when world > 1): a single-GPU / Julia user never loads
@@ -95,10 +92,9 @@ struct sb_ctx {
     cudaStream_t xstream[4] = {nullptr, nullptr, nullptr, nullptr};  // column-exchange streams, one per owner in flight
     sb_timings tm{};
     bool fine_timing = true;
-    int trailing_mode = 0;   // 0: fp64 DMMA (mma.sync), 1: tcgen05 int8 Ozaki slices (ozaki.cu)
-    int num_sms = 148;
-    int oz_mode = SB_DEFAULT_OZ_MODE;  // SB_OZ_MODE=0|2
-    int sweep_variant = 2;      // persistent sweep variant (solve.cu): 2 = diag CTA + L2 prefetch (fastest measured)
+    int trailing_mode = 0;   // 0: fp64 DMMA (mma.sync), 1: int8 Ozaki slices on wgmma (ozaki.cu)
+    int num_sms = 132;
+    int sweep_variant = 2;      // persistent sweep variant (solve.cu): 2 = diag CTA + L2 prefetch
     bool legacy_solve = false;  // SB_SOLVE=legacy: two launches per block instead of the persistent sweep
     cudaEvent_t marks[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
     // peer-to-peer panel exchange over NVLink (multi-GPU, see "P2P panel exchange" below)
@@ -172,7 +168,7 @@ struct sb_factor {
     bool has_alpha = false;
     double logdet = 0.0;
     size_t bytes_L = 0, bytes_invL = 0, bytes_ld = 0, bytes_panel = 0, bytes_alpha = 0, bytes_ldiag = 0;
-    // tcgen05 trailing update (ozaki.cu): two sets (look-ahead) of int8 digit planes + row scales
+    // int8 Ozaki trailing update (ozaki.cu): two sets (look-ahead) of int8 digit planes + row scales
     bool oz = false;
     signed char* oz_planes[2] = {nullptr, nullptr};
     double* oz_scale[2] = {nullptr, nullptr};
@@ -184,10 +180,8 @@ struct sb_factor {
     int* vcache_flag = nullptr;
     bool vcache_valid = false;
     OzMaps oz_maps[2];
-    OzDesc oz_desc;
-    int oz_mode = 0;   // TMA / pipeline variant of the tcgen05 kernel (ozaki.cu: 0 = SW64 x 2 stages, 2 = SW32 x 5 stages)
     size_t bytes_oz_planes = 0;
-    // wide panel phase (tcgen05 path, see wide_panel_phase): dense scratch of the step's 512 x 512 diagonal block
+    // wide panel phase (int8 Ozaki path, see wide_panel_phase): dense scratch of the step's 512 x 512 diagonal block
     // stacked over an identity (input and result copies), inv(L_512) and its digit planes
     bool wide = false;
     double* wide_D = nullptr;        // [2][1024 x 512], ld 1024
@@ -378,8 +372,7 @@ struct CholEv { cudaEvent_t e[4]; };
 // logdet share and the tiled sub-diagonal panel.  Non-owners drop L_kk into their packed matrix, so
 // after the sweep every rank holds the complete factor without any extra collective.
 // ---------------------------------------------------------------------------------------------
-// P2P panel exchange.  Round-2 measurement (2 and 4 GPUs): the 512 NCCL panel broadcasts of a
-// factorisation cost 0.6-1.2 ms each next to the trailing update, because an NCCL broadcast is a
+// P2P panel exchange.  Next to the trailing update an NCCL panel broadcast is slow, because it is a
 // kernel on BOTH sides: the receivers' copies spin on SMs until the owner has factored the panel and
 // the trailing update has to give those SMs up (or the broadcast starves).  The panels are moved
 // by the copy engines instead, with no SM on the receiving side waiting for data:
@@ -614,15 +607,19 @@ static int32_t bcast_panel(sb_ctx* c, sb_factor* f, int64_t k, double* Pslab, si
 constexpr int LOOKAHEAD_SMS = 8;
 constexpr int OZ_CHUNK_TILES = 8;   // tiles per CTA of a chunked T^B launch (multi-GPU default)
 
-// How many SMs T^B leaves to the concurrent panel phase.  Round-2 measurement (4 GPUs): with a fixed 8
-// SMs the panel-phase GEMMs (catch-up SYRK, TRSM-as-GEMM: up to ~2000 DMMA half-tiles per outer step)
-// crawl on 16 CTA slots and the panel chain, not the trailing update, sets the pace of the second half
-// of the factorisation (160 ms of exposed waiting in a 446 ms factorisation).  Pick the reservation that
-// balances  T^B * S/(S-r)  against  serial chain + panel GEMM work / r.
+// How many SMs T^B leaves to the concurrent panel phase.  With a fixed 8 SMs the panel-phase GEMMs
+// (catch-up SYRK, TRSM-as-GEMM: up to ~2000 DMMA half-tiles per outer step) crawl on 16 CTA slots and
+// the panel chain, not the trailing update, can set the pace of the second half of the factorisation.
+// Pick the reservation that balances  T^B * S/(S-r)  against  serial chain + panel GEMM work / r.
+// Per-tile costs: time per SM of one 128 x 64 half-tile with K = 512 (2*128*64*512 flop) at the
+// trailing-update rates bench.py measured at N = 65536 on one H100 80GB (700 W): DMMA 28.1 TFLOP/s,
+// int8 Ozaki 23.0 TFLOP/s fp64-equivalent, over 132 SMs.  The serial-chain and wide-phase latencies
+// below have not been measured on H100.
+constexpr double DMMA_HALF_TILE_US = 39.5, OZ_HALF_TILE_US = 48.1;
 static int pick_lookahead_sms(int num_sms, double tilesB_half, bool oz, int nq_next, int64_t rows_next, int world,
                               bool wide = false) {
-    const double t_tile_us = oz ? 14.5 : 2 * 16.5;                 // per half-tile per SM (measured)
-    const double serial_us = nq_next * (world > 1 ? 230.0 : 150.0); // potrf + (broadcast latency)
+    const double t_tile_us = oz ? OZ_HALF_TILE_US : DMMA_HALF_TILE_US;   // per half-tile per SM
+    const double serial_us = nq_next * (world > 1 ? 230.0 : 150.0); // potrf + (broadcast latency); unmeasured
     // DMMA half-tiles of the next panel phase: TRSM (nq panels) + catch-up (0 + 1 + 2 + 3 segments)
     const double gemm_tiles = (double)nq_next * (rows_next / 64.0) * (1.0 + 0.5 * (nq_next - 1) * 0.5);
     static const int forced = getenv("SB_LOOKAHEAD_SMS") ? atoi(getenv("SB_LOOKAHEAD_SMS")) : 0;
@@ -633,10 +630,11 @@ static int pick_lookahead_sms(int num_sms, double tilesB_half, bool oz, int nq_n
     for (int r : cand) {
         if (r >= num_sms / 2) break;
         const double tB = tilesB_half * t_tile_us / (num_sms - r);
-        // wide phase: ~0.9 ms of potrfs / small products per step, then ONE tcgen05 product of
+        // wide phase: potrfs / small products per step (~0.9 ms assumed), then ONE int8 Ozaki product of
         // (rows / 128) x 8 half-tiles (K = 512) confined to the r free SMs
-        const double tP = wide ? 900.0 + (world > 1 ? 350.0 : 0.0) + (double)(rows_next / NB) * 8.0 * 14.5 / r
-                               : serial_us + gemm_tiles * 8.4 / (2.0 * r);
+        // (panel-phase GEMM tiles have K = 128: a quarter of a half-tile's work)
+        const double tP = wide ? 900.0 + (world > 1 ? 350.0 : 0.0) + (double)(rows_next / NB) * 8.0 * OZ_HALF_TILE_US / r
+                               : serial_us + gemm_tiles * (DMMA_HALF_TILE_US / 4.0) / r;
         const double t = tB > tP ? tB : tP;
         if (t < best_t - 1e-9) { best_t = t; best = r; }
     }
@@ -684,10 +682,9 @@ static int32_t panel_phase(sb_ctx* c, sb_factor* f, int64_t k0, int nq, double* 
 }
 
 // ---------------------------------------------------------------------------------------------
-// Wide panel phase (tcgen05 path).  The per-panel chain  catch-up -> potrf -> TRSM -> exchange  (x 512)
-// keeps full-height DMMA products between the potrfs; measured at 2 / 4 GPUs that chain, squeezed onto the
-// SMs the trailing update leaves free, bounds the factorisation (chain 620 / 415 ms vs trailing 549 /
-// 290 ms).  Here the four block columns of an outer step are factored together:
+// Wide panel phase (int8 Ozaki path).  The per-panel chain  catch-up -> potrf -> TRSM -> exchange  (x 512)
+// keeps full-height DMMA products between the potrfs; on several GPUs that chain, squeezed onto the
+// SMs the trailing update leaves free, can bound the factorisation.  Here the four block columns of an outer step are factored together:
 //   (0) multi-GPU: every owner publishes its (already updated) block column, everyone pulls the other three
 //       into its own packed matrix (copy engines, see "P2P panel exchange") -- all ranks then do the rest
 //       redundantly, so nothing but the raw columns crosses NVLink;
@@ -828,8 +825,8 @@ static int32_t wide_bulk_phase(sb_ctx* c, sb_factor* f, int64_t k0, int nq, int 
     }
     launch_oz_slice(as, 0, below, r0 * NB, Np, f->oz_scale[set], f->oz_expo[set], f->oz_planes[set], st);
     if (launch_panel_solve_ozaki(xcol, ldx, below * NB, &f->oz_maps[set], f->oz_scale[set], r0 * NB, &f->wide_wmaps,
-                                 f->wide_wscale, &f->oz_desc, st) != 0) {
-        sb::set_error("tcgen05 panel solve failed to launch");
+                                 f->wide_wscale, st) != 0) {
+        sb::set_error("int8 Ozaki panel solve failed to launch");
         return SB_ERR_CUDA;
     }
     launch_oz_slice(as, 0, below, r0 * NB, Np, f->oz_scale[set], f->oz_expo[set], f->oz_planes[set], st);
@@ -892,8 +889,8 @@ static int32_t cholesky_lookahead(sb_ctx* c, sb_factor* f, int world, int rank) 
             auto trailing = [&](int64_t jlo, int64_t jhi, int reserve) -> int32_t {
                 if (f->oz) {
                     if (launch_syrk_ozaki(f->L, k0, nq, jlo, jhi, rank, world, &f->oz_maps[set], f->oz_scale[set],
-                                          &f->oz_desc, f->oz_mode, s1, reserve) != 0) {
-                        sb::set_error("tcgen05 trailing kernel could not be launched");
+                                          s1, reserve) != 0) {
+                        sb::set_error("int8 Ozaki trailing kernel could not be launched");
                         return SB_ERR_CUDA;
                     }
                 } else {
@@ -919,7 +916,7 @@ static int32_t cholesky_lookahead(sb_ctx* c, sb_factor* f, int world, int rank) 
                 const double tilesB = 2.0 * (double)syrk_packed_tiles(nblk, k0, jA, nblk, rank, world);
                 const int nq1 = (int)(nblk - jt < OUTER_BLOCKS ? nblk - jt : OUTER_BLOCKS);
                 // T^B next to a panel phase: either a persistent grid that leaves `reserve` SMs free, or
-                // (tcgen05 path, SB_OZ_CHUNK > 0) short-lived CTAs of `chunk` tiles each, which hand SMs to
+                // (int8 Ozaki path, SB_OZ_CHUNK > 0) short-lived CTAs of `chunk` tiles each, which hand SMs to
                 // the high-priority panel stream as they retire.
                 static const int chunk_env = getenv("SB_OZ_CHUNK") ? atoi(getenv("SB_OZ_CHUNK")) : 0;
                 int reserve = (s + 1 < nsteps)
@@ -973,10 +970,10 @@ static int32_t cholesky_lookahead(sb_ctx* c, sb_factor* f, int world, int rank) 
     return SB_OK;
 }
 
-// Factorisation with the wide panel phase (tcgen05 path).  Per outer step s, on the trailing stream:
+// Factorisation with the wide panel phase (int8 Ozaki path).  Per outer step s, on the trailing stream:
 //   T^A_s | T^B_s part 1 (leaves a few SMs free) | panel solve of step s+1 (whole GPU) | T^B_s part 2 (whole GPU)
 // and on the panel stream, under T^B_s part 1: column exchange + diagonal block + inv(L_512) of step s+1.
-// Part 1 is sized to the duration of that serial chain, so the SM reservation costs ~ (8 / 148) x 1 ms per step.
+// Part 1 is sized to the duration of that serial chain, so the SM reservation costs ~ 8 / 132 of the GPU for that long per step.
 static int32_t cholesky_wide(sb_ctx* c, sb_factor* f, int world, int rank) {
     const int64_t nblk = f->L.nblk(), Np = f->Np;
     std::vector<CommEv> comm_ev, chain_ev, bulk_ev;
@@ -1042,9 +1039,9 @@ static int32_t cholesky_wide(sb_ctx* c, sb_factor* f, int world, int rank) {
         if (jt < nblk) {
             const int64_t jA = jt + OUTER_BLOCKS < nblk ? jt + OUTER_BLOCKS : nblk;
             auto trailing = [&](int64_t jlo, int64_t jhi, int reserve, int64_t lo, int64_t hi) -> int32_t {
-                if (launch_syrk_ozaki(f->L, k0, nq, jlo, jhi, rank, world, &f->oz_maps[set], f->oz_scale[set], &f->oz_desc,
-                                      f->oz_mode, s1, reserve, nullptr, lo, hi) != 0) {
-                    sb::set_error("tcgen05 trailing kernel could not be launched");
+                if (launch_syrk_ozaki(f->L, k0, nq, jlo, jhi, rank, world, &f->oz_maps[set], f->oz_scale[set],
+                                      s1, reserve, lo, hi) != 0) {
+                    sb::set_error("int8 Ozaki trailing kernel could not be launched");
                     return SB_ERR_CUDA;
                 }
                 return SB_OK;
@@ -1089,7 +1086,7 @@ static int32_t cholesky_wide(sb_ctx* c, sb_factor* f, int world, int rank) {
             float ms = 0;
             cudaEventElapsedTime(&ms, bulk_ev[i].a, bulk_ev[i].b);
             if (i > 0) bk += ms;               // the first panel solve lies before ev_t0[0]
-            c->tm.panel_ms += ms;              // panel solves are on the critical path (whole GPU, ~0.4 ms each)
+            c->tm.panel_ms += ms;              // panel solves are on the critical path (whole GPU)
         }
         c->tm.trailing_ms += tr - bk;
         c->tm.trailing_kernel_ms += tr - bk;
@@ -1119,10 +1116,9 @@ int32_t cholesky_packed(sb_ctx* c, sb_factor* f, bool force_local = false) {
     const int64_t nblk = f->L.nblk();
     const int world = force_local ? 1 : c->world, rank = force_local ? 0 : c->rank;
     // look-ahead (panel phase of step s+1 on stream 2 under the big trailing update of step s) also
-    // pays on ONE GPU: the serial potrf/TRSM chain (106 ms at N=65536) leaves the critical path
-    // (measured, round 2: with the DMMA trailing kernel on ONE GPU the 8 SMs the look-ahead reserves
-    //  cost as much as the hidden 106 ms panel chain saves, so it is used for world > 1 and for the
-    //  3x faster tcgen05 trailing kernel, where the serial panel chain would be ~10 % of the step)
+    // pays on ONE GPU: the serial potrf/TRSM chain leaves the critical path
+    // (with the DMMA trailing kernel on ONE GPU the 8 SMs the look-ahead reserves cost about as much
+    //  as the hidden panel chain saves, so it is used for world > 1 and for the int8 Ozaki trailing kernel)
     static const bool no_la = getenv("SB_NO_LOOKAHEAD") != nullptr;
     static const bool force_la = getenv("SB_FORCE_LOOKAHEAD") != nullptr;
     if (!no_la && nblk > OUTER_BLOCKS && (world > 1 || f->oz || force_la)) {
@@ -1285,8 +1281,8 @@ int32_t sb_ctx_create(int32_t device, sb_ctx** out) {
     SB_CUDA(cudaSetDevice(device));
     cudaDeviceProp prop;
     SB_CUDA(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10 || prop.minor != 0) {   // the cubin is sm_100a only (sm_103 would fail at the first launch)
-        sb::set_error("libstheno_b200 is built for sm_100a (B200) only; found sm_" +
+    if (prop.major != 9 || prop.minor != 0) {   // the cubin is sm_90a only (wgmma / setmaxnreg have no later-arch form)
+        sb::set_error("libstheno_b200 is built for sm_90a (H100) only; found sm_" +
                       std::to_string(prop.major) + std::to_string(prop.minor));
         return SB_ERR_UNSUPPORTED;
     }
@@ -1302,8 +1298,6 @@ int32_t sb_ctx_create(int32_t device, sb_ctx** out) {
     const char* ft = getenv("SB_FINE_TIMING");
     if (ft && ft[0] == '0') c->fine_timing = false;
     SB_CUDA(cudaDeviceGetAttribute(&c->num_sms, cudaDevAttrMultiProcessorCount, device));
-    const char* om = getenv("SB_OZ_MODE");
-    if (om) { int m = atoi(om); if (m == 0 || m == 2 || m == 4 || m == 6 || m == 8 || m == 10 || m == 16) c->oz_mode = m; }
     const char* sv = getenv("SB_SOLVE");
     c->legacy_solve = sv && !strcmp(sv, "legacy");
     if (sv && !strcmp(sv, "a")) c->sweep_variant = 0;
@@ -1374,13 +1368,12 @@ int32_t sb_ctx_timings(sb_ctx* c, sb_timings* out, int32_t reset) {
 int32_t sb_ctx_set_option(sb_ctx* c, const char* key, int64_t value) {
     SB_CHECK(c && key, "null argument");
     if (!strcmp(key, "trailing")) {
-        SB_CHECK(value == 0 || value == 1, "trailing: 0 = fp64 DMMA, 1 = tcgen05 int8 Ozaki");
+        SB_CHECK(value == 0 || value == 1, "trailing: 0 = fp64 DMMA, 1 = int8 Ozaki");
         c->trailing_mode = (int)value;
         return SB_OK;
     }
     if (!strcmp(key, "fine_timing")) { c->fine_timing = value != 0; return SB_OK; }
     if (!strcmp(key, "sweep_variant")) { c->sweep_variant = (int)value; c->legacy_solve = value < 0; return SB_OK; }
-    if (!strcmp(key, "oz_mode")) { c->oz_mode = (int)value; return SB_OK; }
     sb::set_error(std::string("unknown option ") + key);
     return SB_ERR_INVALID;
 }
@@ -1519,7 +1512,7 @@ static int32_t factor_alloc(sb_ctx* c, int64_t N, sb_factor** out) {
     if (e == cudaSuccess) e = c->pool_alloc((void**)&f->vcache_flag, sizeof(int));
     if (e == cudaSuccess) e = cudaMemsetAsync(f->info_dev, 0, sizeof(long long), c->stream);
     if (e == cudaSuccess) e = cudaMemsetAsync(f->logdet_blk, 0, nblk * sizeof(double), c->stream);
-    // tcgen05 path: worth it (and exercised) once the trailing matrix has a few hundred tiles
+    // int8 Ozaki path: worth it (and exercised) once the trailing matrix has a few hundred tiles
     if (e == cudaSuccess && c->trailing_mode == 1 && nblk > 2 * OUTER_BLOCKS) {
         f->bytes_oz_planes = oz_planes_bytes(f->Np);
         for (int i = 0; i < 2 && e == cudaSuccess; i++) {
@@ -1528,24 +1521,22 @@ static int32_t factor_alloc(sb_ctx* c, int64_t N, sb_factor** out) {
             if (e == cudaSuccess) e = c->pool_alloc((void**)&f->oz_expo[i], (size_t)f->Np * sizeof(int));
         }
         if (e == cudaSuccess) {
-            f->oz_mode = c->oz_mode;
-            oz_default_desc(&f->oz_desc, f->oz_mode);
-            if (oz_make_maps(f->oz_planes[0], f->Np, f->oz_mode, &f->oz_maps[0]) != 0 ||
-                oz_make_maps(f->oz_planes[1], f->Np, f->oz_mode, &f->oz_maps[1]) != 0) {
+            if (oz_make_maps(f->oz_planes[0], f->Np, &f->oz_maps[0]) != 0 ||
+                oz_make_maps(f->oz_planes[1], f->Np, &f->oz_maps[1]) != 0) {
                 sb_factor_destroy(f);
                 sb::set_error("cuTensorMapEncodeTiled failed for the int8 digit planes");
                 return SB_ERR_CUDA;
             }
             f->oz = true;
             static const bool no_wide = getenv("SB_WIDE_PANEL") && getenv("SB_WIDE_PANEL")[0] == '0';
-            if (!no_wide && (f->oz_mode >= 16 || (f->oz_mode & 3) == 0)) {   // the panel solve instance needs SWIZZLE_64B maps
+            if (!no_wide) {
                 constexpr int64_t WD = (int64_t)OUTER_BLOCKS * NB;
                 e = c->pool_alloc((void**)&f->wide_D, (size_t)2 * 2 * WD * WD * sizeof(double));
                 if (e == cudaSuccess) e = c->pool_alloc((void**)&f->wide_W, (size_t)WD * WD * sizeof(double));
                 if (e == cudaSuccess) e = c->pool_alloc((void**)&f->wide_wp, oz_planes_bytes(WD));
                 if (e == cudaSuccess) e = c->pool_alloc((void**)&f->wide_wscale, (size_t)WD * sizeof(double));
                 if (e == cudaSuccess) e = c->pool_alloc((void**)&f->wide_wexpo, (size_t)WD * sizeof(int));
-                if (e == cudaSuccess && oz_make_maps(f->wide_wp, WD, f->oz_mode, &f->wide_wmaps) != 0) {
+                if (e == cudaSuccess && oz_make_maps(f->wide_wp, WD, &f->wide_wmaps) != 0) {
                     sb_factor_destroy(f);
                     sb::set_error("cuTensorMapEncodeTiled failed for the inv(L_512) digit planes");
                     return SB_ERR_CUDA;
@@ -1801,19 +1792,19 @@ int32_t sb_factor_alpha(sb_ctx* c, sb_factor* f, void* alpha_out) {
     return SB_OK;
 }
 
-// workspace of the tcgen05 matrix-TRSM sweep: digit planes / scales / tensor maps of the X panels
+// workspace of the int8 Ozaki matrix-TRSM sweep: digit planes / scales / tensor maps of the X panels
 struct OzSweepWs {
     DevBuf planes, scale, expo;
     OzMaps maps;
     int64_t rows = 0;
     bool ready = false;
     explicit OzSweepWs(sb_ctx* c) : planes(c), scale(c), expo(c) {}
-    int32_t init(int64_t rows_p, int mode) {
+    int32_t init(int64_t rows_p) {
         rows = rows_p;
         SB_TRY(planes.alloc(oz_planes_bytes(rows_p)));
         SB_TRY(scale.alloc(rows_p * sizeof(double)));
         SB_TRY(expo.alloc(rows_p * sizeof(int)));
-        if (oz_make_maps(reinterpret_cast<signed char*>(planes.p), rows_p, mode, &maps) != 0) {
+        if (oz_make_maps(reinterpret_cast<signed char*>(planes.p), rows_p, &maps) != 0) {
             sb::set_error("cuTensorMapEncodeTiled failed for the X digit planes");
             return SB_ERR_CUDA;
         }
@@ -1825,7 +1816,7 @@ constexpr int SWEEP_COLS = OUTER_BLOCKS * NB;  // columns of the Xk workspace (r
 
 // W <- W L^{-T} (rows_p x Np, ld rows_p): right-looking block forward substitution, tensor-core
 // products only.  keep: write the result back into W; acc != null: acc[r] += sum_c result[r,c]^2.
-// Xk: rows_p x 512 workspace.  With a tcgen05-enabled factor (f->oz) the big update of each outer
+// Xk: rows_p x 512 workspace.  With a int8-Ozaki factor (f->oz) the big update of each outer
 // step (4 block columns, K = 512) runs on the int8 Ozaki kernel; the small in-step products stay DMMA.
 static int32_t trsm_sweep(sb_ctx* c, sb_factor* f, double* W, int64_t rows_p, double* Xk, bool keep, double* acc,
                           OzSweepWs* ws = nullptr) {
@@ -1860,8 +1851,8 @@ static int32_t trsm_sweep(sb_ctx* c, sb_factor* f, double* W, int64_t rows_p, do
                             reinterpret_cast<signed char*>(ws->planes.p), c->stream);
             launch_oz_slice(sl, 0, m / NB, jt * (int64_t)NB, Np, f->oz_scale[0], f->oz_expo[0], f->oz_planes[0], c->stream);
             if (launch_gemm_ozaki(W + jt * NB * rows_p, rows_p, rows_p, m, nq, &ws->maps, ws->scale.d(), 0, &f->oz_maps[0],
-                                  f->oz_scale[0], jt * (int64_t)NB, &f->oz_desc, f->oz_mode, c->stream) != 0) {
-                sb::set_error("tcgen05 sweep kernel could not be launched");
+                                  f->oz_scale[0], jt * (int64_t)NB, c->stream) != 0) {
+                sb::set_error("int8 Ozaki sweep kernel could not be launched");
                 return SB_ERR_CUDA;
             }
         }
@@ -1956,7 +1947,7 @@ static int32_t predict_impl(sb_ctx* c, sb_factor* f, const sb_covspec* cross,
         SB_CUDA(cudaMemsetAsync(acc.p, 0, Nsp * sizeof(double), c->stream));
         // V^T = W L^{-T}: block forward substitution from the right, tensor-core products only
         OzSweepWs ws(c);
-        if (f->oz) SB_TRY(ws.init(Nsp, f->oz_mode));
+        if (f->oz) SB_TRY(ws.init(Nsp));
         SB_TRY(trsm_sweep(c, f, W.d(), Nsp, Xk.d(), /*keep=*/full_cov, full_cov ? nullptr : acc.d(), &ws));
         if (!full_cov) {
             SB_TRY(pd.alloc(Nsp * sizeof(double)));
@@ -2079,7 +2070,7 @@ int32_t sb_logpdf_grad(sb_ctx* c, sb_factor* f, const sb_covspec* spec, double* 
     SB_CUDA(cudaMemsetAsync(g.p, 0, (size_t)2 * (spec->nterms > 0 ? spec->nterms : 1) * sizeof(double), c->stream));
     set_identity_kernel<<<(unsigned)((Np + 255) / 256), 256, 0, c->stream>>>(W.d(), Np);
     OzSweepWs ws(c);
-    if (f->oz) SB_TRY(ws.init(Np, f->oz_mode));
+    if (f->oz) SB_TRY(ws.init(Np));
     SB_TRY(trsm_sweep(c, f, W.d(), Np, Xk.d(), /*keep=*/true, nullptr, &ws));              // W = L^{-T}
     launch_gemm_nt(W.d(), Np, W.d(), Np, Kinv.d(), Np, Np, Np, Np, 1.0, 0.0, c->stream);  // K^{-1} = W W'
     for (auto& b : ds.blocks) {
@@ -2222,7 +2213,7 @@ int32_t sb_vfe_create(sb_ctx* c, const sb_covspec* uu, const sb_noise* noise_u, 
     VFE_CUDA(cudaMemsetAsync(fro.p, 0, (size_t)(nchunks_total + 1) * sizeof(double), c->stream));
 
     OzSweepWs ws(c);
-    if (v->fu->oz) VFE_TRY(ws.init(NC, v->fu->oz_mode));
+    if (v->fu->oz) VFE_TRY(ws.init(NC));
     for (int64_t ci = c->rank; ci < nchunks_total; ci += c->world) {  // chunks round-robin over ranks
         const int64_t r0 = ci * NC, r1 = r0 + NC < N ? r0 + NC : N;
         const int64_t rows = r1 - r0, rows_p = round_up(rows, NB);
@@ -2314,7 +2305,7 @@ int32_t sb_vfe_predict_cov(sb_ctx* c, sb_vfe* v, const sb_covspec* cross, const 
     SB_TRY(assemble_dense(c, dc, W.d(), Nsp));
     SB_TRY(assemble_dense(c, dp, Cm.d(), Nsp));
     OzSweepWs ws(c);
-    if (v->fu->oz || v->fl->oz) SB_TRY(ws.init(Nsp, v->fu->oz ? v->fu->oz_mode : v->fl->oz_mode));
+    if (v->fu->oz || v->fl->oz) SB_TRY(ws.init(Nsp));
     SB_TRY(trsm_sweep(c, v->fu, W.d(), Nsp, Xk.d(), true, nullptr, &ws));      // W = B'
     launch_gemm_nt(W.d(), Nsp, W.d(), Nsp, Cm.d(), Nsp, Nsp, Nsp, Mp, -1.0, 1.0, c->stream);
     SB_TRY(trsm_sweep(c, v->fl, W.d(), Nsp, Xk.d(), true, nullptr, &ws));      // W = (L_Lambda^{-1} B)'
@@ -2358,7 +2349,7 @@ int32_t sb_vfe_predict(sb_ctx* c, sb_vfe* v, const sb_covspec* cross, const sb_c
         SB_CUDA(cudaMemsetAsync(pd.p, 0, Nsp * sizeof(double), c->stream));
         // B^T = K_*u L_u^{-T} (kept), then (L_Lambda^{-1} B)^T = B^T L_Lambda^{-T}
         OzSweepWs ws(c);
-        if (v->fu->oz || v->fl->oz) SB_TRY(ws.init(Nsp, v->fu->oz ? v->fu->oz_mode : v->fl->oz_mode));
+        if (v->fu->oz || v->fl->oz) SB_TRY(ws.init(Nsp));
         SB_TRY(trsm_sweep(c, v->fu, W.d(), Nsp, Xk.d(), true, acc1.d(), &ws));
         SB_TRY(trsm_sweep(c, v->fl, W.d(), Nsp, Xk.d(), false, acc2.d(), &ws));
         SB_TRY(assemble_diag(c, dp, pd.d()));

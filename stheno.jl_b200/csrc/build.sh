@@ -1,12 +1,13 @@
 #!/bin/bash
-# Build libstheno_b200.so (sm_100a only) in-tree: stheno.jl_b200/libstheno_b200.so
+# Build libstheno_b200.so (sm_90a only) in-tree: stheno.jl_b200/libstheno_b200.so
 set -e
 cd "$(dirname "$0")"
 NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
-FLAGS="-gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-O2 -Xptxas -v"
+ARCH="-gencode arch=compute_90a,code=sm_90a"
+FLAGS="$ARCH -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-O2 -Xptxas -v"
 mkdir -p ../../build
 for f in assemble gemm_nt ozaki potrf solve api; do
   $NVCC $FLAGS -c $f.cu -o ../../build/$f.o 2> ../../build/$f.ptxas.log || { cat ../../build/$f.ptxas.log; exit 1; }
 done
-$NVCC -shared -o ../libstheno_b200.so ../../build/assemble.o ../../build/gemm_nt.o ../../build/ozaki.o ../../build/potrf.o ../../build/solve.o ../../build/api.o -lcudart -ldl
+$NVCC $ARCH -shared -o ../libstheno_b200.so ../../build/assemble.o ../../build/gemm_nt.o ../../build/ozaki.o ../../build/potrf.o ../../build/solve.o ../../build/api.o -lcudart -ldl
 echo "built $(cd ..; pwd)/libstheno_b200.so"

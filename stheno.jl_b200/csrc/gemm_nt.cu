@@ -6,7 +6,7 @@
 // It replaces LAPACK dpotrf's dsyrk/dgemm/dtrsm inside `cholesky(Symmetric(K + Sigma_y))` and
 // the `C.U' \ K_fx` solves of AbstractGPs (SURVEY.md App. A).
 //
-// sm_100a notes.  tcgen05.mma has no fp64 kind, so fp64 tensor math is the DMMA path
+// sm_90a notes.  wgmma has no fp64 kind, so fp64 tensor math is the DMMA path
 // (mma.sync.m8n8k4.f64 -> SASS DMMA.8x8x4).  Operand k-slabs are staged global->shared by the
 // TMA engine with 1-D bulk copies (cp.async.bulk ... mbarrier::complete_tx -> SASS UBLKCP) into a
 // 4-stage ring; one mbarrier per stage.  Shared tiles are [k][row] with a 4-double pad so the
@@ -168,7 +168,7 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 // warps 0..7 are math warps (LDS.64 fragments + DMMA + epilogue, no copy-issue code at all);
 // warp 8 is the TMA producer: its lane 0 runs the whole refill loop (wait empty[] -> proxy fence
 // -> arm full[] with the slab's byte count -> 32 bulk copies).  Issuing bulk copies from the math
-// warps cost 12 % of the tensor pipe (ablation in profiles/): a UBLKCP stalls its warp ~30 ns.
+// warps costs tensor-pipe issue slots: a bulk-copy issue stalls its warp.
 // The ring is addressed by a chunk counter that runs ACROSS tiles, so the next tile's first
 // k-slabs are already landing while the math warps are in the current tile's epilogue.  No
 // CTA-wide barrier in steady state: full[] (tx-count) / empty[] (8 warp arrivals) mbarriers only.

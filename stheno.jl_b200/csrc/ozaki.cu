@@ -1,26 +1,25 @@
-// K3': fp64 trailing update on the 5th-generation tensor cores (tcgen05 + TMEM) by integer slicing.
+// K3': fp64 trailing update on the int8 tensor cores (Hopper wgmma) by integer slicing.
 //
-// tcgen05.mma has no fp64 kind; the legacy DMMA path tops out at 37 TFLOP/s on B200.  The only way
-// past that ceiling is the Ozaki scheme on the int8 kind (4.5 POP/s dense on sm_100a): every row
-// of an operand panel is scaled by a power of two and cut into S = 7 signed 8-bit digits
+// The Ozaki scheme on the s8 kind of wgmma: every row of an operand panel is scaled by a power of two
+// and cut into S = 7 signed 8-bit digits
 //      x_ik  ~=  2^(e_i - 55) * sum_{p=1..7} d_p[i,k] * 2^(8(7-p)),     d_p in [-128, 127]
 // (the bytes of the 56-bit two's-complement fixed-point value, re-centred so every digit is
 // balanced), and   sum_k x_ik x_jk = s_i s_j * sum_{t=2..8} 2^(8(8-t)) G_t,   s = 2^(e-31),
 //      G_t[i,j] = sum_{p+q=t} sum_k d_p[i,k] d_q[j,k]
 // is EXACT int32 arithmetic on the tensor cores (|G_t| <= 7 * 512 * 2^14 < 2^31).  Digit pairs with
 // p+q > 8 are dropped: a zero-mean truncation of ~1e-15 relative to |row_i|_max |row_j|_max, i.e.
-// fp64-level.  28 int8 MMAs replace one fp64 MMA and still run ~3x faster than DMMA.
+// fp64-level.  28 int8 MMAs replace one fp64 MMA.
 //
-// Kernel structure (one persistent CTA per SM, 10 warps, warp-specialised):
-//   warp 8  TMA producer: cp.async.bulk.tensor (tensor-map TMA, SASS UTMALDG) of the 7 digit
-//           planes of a 64-byte k-chunk of A (128 rows) and B (64 rows) into a 2-stage smem ring,
-//           128B-free SWIZZLE_64B layout, completion on mbarriers.
-//   warp 9  MMA issuer: one elected lane issues tcgen05.mma.kind::i8 (M=128, N=64, K=32), 56 per
-//           k-chunk, accumulating the seven G_t in seven 64-column TMEM accumulators (448 of the
-//           512 columns); tcgen05.commit releases smem stages and publishes finished accumulators.
-//   warps 0-7 epilogue: tcgen05.ld the int32 accumulators, convert + weight into fp64 registers,
-//           release each TMEM accumulator as soon as it is read (so the next tile's MMAs overlap the
-//           rest of the epilogue), then C -= s_i s_j * acc on the packed fp64 matrix.
+// Kernel structure (persistent CTAs, 3 warpgroups, warp-specialised), one 128 x 64 tile of C at a time:
+//   warps 8-11 producer warpgroup (registers handed to the consumers with setmaxnreg); one lane is the TMA: cp.async.bulk.tensor of the digit planes of a 64-byte k-chunk of A (128
+//              rows) and B (64 rows), one plane per copy, into a 2-stage shared-memory ring in the
+//              SWIZZLE_64B layout wgmma reads; completion on mbarriers.
+//   warps 0-7  two consumer warpgroups, rows 0-63 / 64-127 of the tile: wgmma.m64n64k32.s32.s8.s8
+//              with both operands in shared memory, int32 accumulators in registers.
+// The seven 64x64 int32 accumulators of a warpgroup would take 224 registers per thread, so every tile
+// is computed in two passes over K: pass 0 forms G_2..G_5 (digit planes 1..4 only), pass 1 G_6..G_8 (all
+// planes).  After each pass the accumulators are weighted into fp64 registers in the order t = 2..8,
+// then C -= s_i s_j acc on the packed fp64 matrix.
 // Replaces the dsyrk/dgemm inside LAPACK dpotrf (AbstractGPs `cholesky(Symmetric(cov(fx)))`).
 #include <cuda.h>
 
@@ -31,25 +30,18 @@ namespace {
 
 constexpr int OZ_S = 7;              // digit planes
 constexpr int OZ_BM = 128, OZ_BN = 64;
-constexpr int OZ_THREADS = 320;
-constexpr int OZ_EPI_WARPS = 8;
 constexpr int OZ_KMAX = 512;         // bytes of K per row in the digit planes (row pitch)
-
-// Pipeline shape: KC = bytes of K per smem stage, STAGES = ring depth.  The MMA floor is 7.5 us per
-// 128x64x512 tile and a tile needs 688 KB of operands, i.e. ~92 GB/s per SM: with ~1-2 us of TMA
-// latency the ring must keep >= 100-180 KB in flight.  (KC=64, 2 stages) keeps only 84 KB in flight
-// and measured 19.6 us/tile (ncu: tensor pipe 39 %, profiles/ncu_ozaki_r2.txt); (KC=32, 5 stages)
-// keeps 168 KB in flight inside the same shared memory.
-template <int KC, int STAGES>
-struct OzCfg {
-    static constexpr int A_PLANE = OZ_BM * KC;
-    static constexpr int B_PLANE = OZ_BN * KC;
-    static constexpr int A_STAGE = OZ_S * A_PLANE;
-    static constexpr int B_STAGE = OZ_S * B_PLANE;
-    static constexpr int STAGE_BYTES = A_STAGE + B_STAGE;
-    static constexpr int BAR_BYTES = 16 * STAGES + 16 * OZ_S + 16;
-    static constexpr size_t SMEM = (size_t)STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
-};
+constexpr int OZ_KC = 64;            // bytes of K per pipeline stage: one SWIZZLE_64B row
+constexpr int OZ_STAGES = 2;
+constexpr int OZ_MMA_WARPS = 8;      // two consumer warpgroups
+constexpr int OZ_THREADS = OZ_MMA_WARPS * 32 + 128;   // + one producer warpgroup (setmaxnreg works per warpgroup)
+constexpr int OZ_PRODUCER_REGS = 40, OZ_CONSUMER_REGS = 232;   // 128 x 40 + 256 x 232 <= 64K registers
+constexpr int OZ_A_PLANE = OZ_BM * OZ_KC;                        // 8 KB
+constexpr int OZ_B_PLANE = OZ_BN * OZ_KC;                        // 4 KB
+constexpr int OZ_A_STAGE = OZ_S * OZ_A_PLANE;
+constexpr int OZ_STAGE_BYTES = OZ_S * (OZ_A_PLANE + OZ_B_PLANE);  // 84 KB
+constexpr size_t OZ_SMEM = (size_t)OZ_STAGES * OZ_STAGE_BYTES + 1024 /*align*/ + 64 /*barriers*/;
+constexpr int OZ_PASS0_GROUPS = 4;   // pass 0: G_2..G_5 from planes 1..4; pass 1: G_6..G_8 from all 7
 
 struct OzArgs {
     int mode;         // 1: packed SYRK (A == B == the panel), 0: plain  C[M x Ncols] -= A B^T, dense C
@@ -59,7 +51,7 @@ struct OzArgs {
     int64_t tile_lo, tile_hi;   // this launch covers tiles [tile_lo, tile_hi) of the list (a trailing update can be split)
     int tri;             // plain mode: B is block lower triangular (128-blocks): column block q only needs K <= 128 (q + 1)
     int tiles_per_cta;   // 0: persistent CTAs (tile t = blockIdx.x + i*gridDim.x); > 0: CTA b owns tiles [b*tpc, (b+1)*tpc)
-    int kchunks;      // K / KC
+    int kchunks;      // K / OZ_KC
     const double* scaleA;  // row scales s_i = 2^(e_i - 31), indexed by plane row of A / B
     const double* scaleB;
     // plain mode: tile (rt, ct) = (t % mtiles, t / mtiles); plane rows rowA0 + 128 rt, rowB0 + 64 ct
@@ -67,18 +59,11 @@ struct OzArgs {
     int64_t ldc, mtiles;
     int64_t rowA0, rowB0;
     // plain mode C addressing: tile (rt, ct) starts at C + rt*c_rt_stride + (ct/2)*c_pair_stride + (ct%2)*64*ldc
-    // (dense column-major: 128, 128*ldc; TILED Cholesky panels: 128*132, distance between panel buffers, ldc 132)
     int64_t c_rt_stride, c_pair_stride;
-    int store;        // 0: C -= s_i s_j acc;  1 (separate kernel instance): C = + s_i s_j acc, no read, and
-                      // column block q = ct / 2 of C has its own base / leading dimension (the packed matrix's block columns)
+    // store instance (panel solve): C = + s_i s_j acc, no read, and column block q = ct / 2 of C has its
+    // own base / leading dimension (the packed matrix's block columns)
     double* cb[4];
     int64_t cld[4];
-    // shared-memory matrix descriptor fields (runtime so the test harness can probe encodings)
-    uint32_t a_kk_adv, b_kk_adv;  // start-address advance (16-byte units) per K=32 step
-    uint32_t a_lbo, b_lbo, sbo;   // 16-byte units
-    uint32_t layout;              // 3-bit layout_type (4 = SWIZZLE_64B, 0 = none)
-    int tma_mode;                 // 0: 3-D SWIZZLE_64B box (KC 64), 1: 4-D un-swizzled interleave (KC 64), 2: 3-D SWIZZLE_32B (KC 32)
-    int* dbg;                     // optional: raw int32 accumulators of tile 0  [7][128][64]
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -92,7 +77,7 @@ __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
-// Spin with a watchdog: a protocol bug must trap (error returned to the caller), never hang the box.
+// Spin with a watchdog: a protocol bug must trap (error returned to the caller), never hang the device.
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     uint32_t ok = 0;
     long long t0 = 0;
@@ -117,90 +102,36 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* tm,
         ::"r"(dst), "l"(tm), "r"(c0), "r"(c1), "r"(c2), "r"(bar)
         : "memory");
 }
-__device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* tm, int c0, int c1, int c2, int c3,
-                                            uint32_t bar) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];"
-        ::"r"(dst), "l"(tm), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(bar)
-        : "memory");
+
+// wgmma shared-memory matrix descriptor of a K-major SWIZZLE_64B operand (the layout the TMA box writes):
+// start address >> 4 at [0,14), leading byte offset (unused when swizzled: 1) at [16,30), stride byte
+// offset 512 B (8 rows x 64 B) >> 4 at [32,46), layout type 2 = 64B swizzle at [62,64)
+__device__ __forceinline__ uint64_t wg_desc(uint32_t saddr) {
+    return (uint64_t)((saddr >> 4) & 0x3fff) | ((uint64_t)1 << 16) | ((uint64_t)32 << 32) | ((uint64_t)2 << 62);
 }
 
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
 
-// D[tmem] (+)= A[smem] * B[smem]^T, int8 x int8 -> int32, M=128 N=64 K=32
-__device__ __forceinline__ void mma_i8(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
+// d[64 x 64] += A[64 x 32 B] * B[64 x 32 B]^T, int8 x int8 -> int32, one warpgroup
+__device__ __forceinline__ void wgmma_s8(int (&d)[32], uint64_t da, uint64_t db) {
     asm volatile(
-        "{\n .reg .pred p;\n setp.ne.b32 p, %4, 0;\n"
-        " tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n}"
-        ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc)
-        : "memory");
-}
-// same, with the two 64-bit shared-memory descriptors assembled from a per-operand low word
-// (start address >> 4 | LBO << 16) and a common compile-time high word (SBO | version | layout):
-// the issue loop then costs one 32-bit add per operand, all in the uniform datapath.
-__device__ __forceinline__ void mma_i8_lohi(uint32_t d_tmem, uint32_t alo, uint32_t blo, uint32_t hi, uint32_t idesc,
-                                            uint32_t acc) {
-    asm volatile(
-        "{\n .reg .pred p;\n .reg .b64 da, db;\n setp.ne.b32 p, %5, 0;\n"
-        " mov.b64 da, {%1, %3};\n mov.b64 db, {%2, %3};\n"
-        " tcgen05.mma.cta_group::1.kind::i8 [%0], da, db, %4, p;\n}"
-        ::"r"(d_tmem), "r"(alo), "r"(blo), "r"(hi), "r"(idesc), "r"(acc)
-        : "memory");
-}
-// A operand from TMEM (tcgen05.mma ".ts" form): A[128 x 32 B] sits in 8 TMEM columns, lane = row
-__device__ __forceinline__ void mma_i8_ts(uint32_t d_tmem, uint32_t a_tmem, uint32_t blo, uint32_t hi, uint32_t idesc,
-                                          uint32_t acc) {
-    asm volatile(
-        "{\n .reg .pred p;\n .reg .b64 db;\n setp.ne.b32 p, %5, 0;\n"
-        " mov.b64 db, {%2, %3};\n"
-        " tcgen05.mma.cta_group::1.kind::i8 [%0], [%1], db, %4, p;\n}"
-        ::"r"(d_tmem), "r"(a_tmem), "r"(blo), "r"(hi), "r"(idesc), "r"(acc)
-        : "memory");
-}
-// shared memory -> TMEM copy of one 128-row x 256-bit operand slab (same matrix descriptor as the MMA's)
-__device__ __forceinline__ void tmem_cp_128x256b(uint32_t dst_tmem, uint32_t slo, uint32_t hi) {
-    asm volatile(
-        "{\n .reg .b64 ds;\n mov.b64 ds, {%1, %2};\n"
-        " tcgen05.cp.cta_group::1.128x256b [%0], ds;\n}"
-        ::"r"(dst_tmem), "r"(slo), "r"(hi)
-        : "memory");
-}
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile("{\n .reg .pred p;\n elect.sync _|p, 0xffffffff;\n selp.u32 %0, 1, 0, p;\n}" : "=r"(pred));
-    return pred != 0;
-}
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-
-// thread <-> its own TMEM lane, 32 consecutive 32-bit columns
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, int (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
+        "wgmma.mma_async.sync.aligned.m64n64k32.s32.s8.s8 "
         "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-          "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-          "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr)
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, 1;"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
+          "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]),
+          "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
+          "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
+        : "l"(da), "l"(db)
         : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
 }
 
-// same enumeration as gemm_nt.cu's packed-SYRK cursor: owned block columns J0, J0+w, ...; column J
-// holds nblk-J row blocks, two 64-wide half tiles per block
 // Tile range of this CTA.  Persistent mode strides the whole list by gridDim.x; chunked mode gives every
 // CTA a short contiguous run and lets the CTA retire, so that kernels of a higher-priority stream (the
 // look-ahead panel phase and its NCCL broadcast) get SMs within microseconds instead of waiting for a
-// persistent grid to finish (round-2 measurement: 0.6-1.2 ms per panel broadcast next to a persistent T^B).
-#ifdef OZ_EXP_NO_CHUNK
-__device__ __forceinline__ int64_t oz_t_begin(const OzArgs& g) { return g.tile_lo + (int64_t)blockIdx.x; }
-__device__ __forceinline__ int64_t oz_t_end(const OzArgs& g) { return g.tile_hi; }
-__device__ __forceinline__ int64_t oz_t_step(const OzArgs& g) { return (int64_t)gridDim.x; }
-#else
+// persistent grid to finish.
 __device__ __forceinline__ int64_t oz_t_begin(const OzArgs& g) {
     return g.tile_lo + (g.tiles_per_cta > 0 ? (int64_t)blockIdx.x * g.tiles_per_cta : (int64_t)blockIdx.x);
 }
@@ -210,14 +141,12 @@ __device__ __forceinline__ int64_t oz_t_end(const OzArgs& g) {
     return e < g.tile_hi ? e : g.tile_hi;
 }
 __device__ __forceinline__ int64_t oz_t_step(const OzArgs& g) { return g.tiles_per_cta > 0 ? 1 : (int64_t)gridDim.x; }
-#endif
 
-// K chunks of tile t (KC bytes each): all of K, or -- triangular B -- only the blocks up to the tile's column block
-template <int KC>
+// K chunks of tile t: all of K, or -- triangular B -- only the blocks up to the tile's column block
 __device__ __forceinline__ int oz_tile_kchunks(const OzArgs& g, int64_t t) {
     if (!g.tri) return g.kchunks;
     const int64_t ct = t / g.mtiles;
-    return (int)((ct >> 1) + 1) * (NB / KC);
+    return (int)((ct >> 1) + 1) * (NB / OZ_KC);
 }
 
 struct OzTile {
@@ -226,6 +155,8 @@ struct OzTile {
     int64_t ldc;
 };
 
+// same enumeration as gemm_nt.cu's packed-SYRK cursor: owned block columns J0, J0+w, ...; column J
+// holds nblk-J row blocks, two 64-wide half tiles per block
 struct OzCursor {
     int64_t t, J, s0;
     __device__ __forceinline__ void init(const OzArgs& g, int64_t t0) {
@@ -265,451 +196,139 @@ struct OzCursor {
     }
 };
 
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo, uint32_t sbo, uint32_t layout) {
-    // tcgen05 shared-memory matrix descriptor: start address [0,14) (>>4), leading byte offset
-    // [16,30) (>>4), stride byte offset [32,46) (>>4), version = 1 at [46,48), layout type [61,64)
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr >> 4) & 0x3fff);
-    d |= (uint64_t)(lbo & 0x3fff) << 16;
-    d |= (uint64_t)(sbo & 0x3fff) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)(layout & 7) << 61;
-    return d;
-}
-
-// Epilogue of both kernel variants (warps 0..7): drain the seven int32 accumulators of each tile from
-// TMEM, weight + sum them in fp64 registers, release each accumulator right after its tcgen05.ld, then
-// C -= s_i s_j acc on the fp64 matrix.
-template <bool STORE>
-__device__ __forceinline__ void oz_epilogue(const OzArgs& g, uint32_t tmem, uint32_t tfull0, uint32_t tempty0, int warp,
-                                            int lane) {
-        const int lq = warp & 3, ch = warp >> 2;  // TMEM lane quarter (hardware: warp % 4), column half
-        OzCursor cur;
-        cur.init(g, oz_t_begin(g));
-        uint32_t it = 0;
-        const int64_t t_end = oz_t_end(g), t_step = oz_t_step(g);
-        for (; cur.t < t_end; cur.advance(g, t_step), it++) {
-            const OzTile tl = cur.tile(g);
-            double acc[32];
+// One pass of a consumer warpgroup over the K chunks of a tile: the groups G_{2+G0} .. G_{1+G1} of its
+// 64 x 64 quarter (digit planes 0 .. G1-1 of both operands), then acc += 2^(8(6-grp)) G_{grp+2} in group order.
+template <int G0, int G1>
+__device__ __forceinline__ void oz_pass(double (&acc)[32], int kch, uint32_t& n, uint32_t base, uint32_t full0,
+                                        uint32_t empty0, int wg, int lane) {
+    int d[G1 - G0][32];
 #pragma unroll
-            for (int c = 0; c < 32; c++) acc[c] = 0.0;
+    for (int i = 0; i < G1 - G0; i++)
 #pragma unroll
-            for (int grp = 0; grp < OZ_S; grp++) {
-                mbar_wait(tfull0 + 8 * grp, it & 1);
-                tc_fence_after();
-                int v[32];
-                tmem_ld32(tmem + ((uint32_t)(lq * 32) << 16) + (uint32_t)(grp * OZ_BN + ch * 32), v);
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(tempty0 + 8 * grp);   // accumulator may be overwritten
-                const double wt = (double)(1ull << (8 * (OZ_S - 1 - grp)));   // 2^(8(8 - t)), t = grp + 2
-                if (g.dbg != nullptr && cur.t == 0) {
+        for (int c = 0; c < 32; c++) d[i][c] = 0;
+    for (int kc = 0; kc < kch; kc++, n++) {
+        const uint32_t st = n % OZ_STAGES, ph = (n / OZ_STAGES) & 1;
+        mbar_wait(full0 + 8 * st, ph);
+        const uint32_t sA = base + st * OZ_STAGE_BYTES + (uint32_t)wg * (64 * OZ_KC), sB = base + st * OZ_STAGE_BYTES + OZ_A_STAGE;
+        wg_fence();
 #pragma unroll
-                    for (int c = 0; c < 32; c++) g.dbg[(grp * OZ_BM + lq * 32 + lane) * OZ_BN + ch * 32 + c] = v[c];
+        for (int kk = 0; kk < OZ_KC / 32; kk++) {
+#pragma unroll
+            for (int grp = G0; grp < G1; grp++) {
+#pragma unroll
+                for (int p = 0; p <= grp; p++) {   // digit planes p (of A) and q = grp - p (of B)
+                    const int q = grp - p;
+                    wgmma_s8(d[grp - G0], wg_desc(sA + p * OZ_A_PLANE + kk * 32), wg_desc(sB + q * OZ_B_PLANE + kk * 32));
                 }
-#ifndef OZ_ABLATE_NO_CVT
-#pragma unroll
-                for (int c = 0; c < 32; c++) acc[c] = fma((double)v[c], wt, acc[c]);
-#else
-                acc[grp] += (double)v[grp] * wt;   // timing experiment: no per-element int -> fp64 work
-#endif
-            }
-            // C[rows lq*32 + lane, cols ch*32 .. +32 of the tile] -= s_i s_j acc
-            const int64_t ldc = tl.ldc;
-            const int row = lq * 32 + lane;
-            double* cp = tl.C + (int64_t)(ch * 32) * ldc + row;
-            const double si = g.scaleA[tl.rowA + row];
-            const double* sj = g.scaleB + tl.rowB + ch * 32;
-#ifdef OZ_ABLATE_NO_C
-            continue;
-#endif
-            if constexpr (STORE) {   // panel solve X = A W^T written straight into the packed matrix: no read of C
-                const int64_t rt = cur.t % g.mtiles, ct = cur.t / g.mtiles;
-                const int64_t ldq = g.cld[ct >> 1];
-                double* xp = g.cb[ct >> 1] + ((ct & 1) * OZ_BN + ch * 32) * ldq + rt * OZ_BM + row;
-#pragma unroll
-                for (int c = 0; c < 32; c++) xp[(int64_t)c * ldq] = (si * sj[c]) * acc[c];
-                continue;
-            }
-#pragma unroll
-            for (int c0 = 0; c0 < 32; c0 += 8) {
-                double old[8];
-#pragma unroll
-                for (int c = 0; c < 8; c++) old[c] = __ldcs(cp + (int64_t)(c0 + c) * ldc);
-#pragma unroll
-                for (int c = 0; c < 8; c++) cp[(int64_t)(c0 + c) * ldc] = fma(-(si * sj[c0 + c]), acc[c0 + c], old[c]);
             }
         }
+        wg_commit();
+        wg_wait_all();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(empty0 + 8 * st);   // this warp no longer reads the stage
+    }
+#pragma unroll
+    for (int grp = G0; grp < G1; grp++) {
+        const double wt = (double)(1ull << (8 * (OZ_S - 1 - grp)));   // 2^(8(8 - t)), t = grp + 2
+#pragma unroll
+        for (int c = 0; c < 32; c++) acc[c] = fma((double)d[grp - G0][c], wt, acc[c]);
+    }
 }
 
-template <int KC, int STAGES, int TMODE, bool ATMEM, bool PAIR, bool STORE = false>
+template <bool STORE>
 __global__ void __launch_bounds__(OZ_THREADS, 1)
 ozaki_syrk_kernel(const __grid_constant__ OzArgs g, const __grid_constant__ CUtensorMap tmA,
                   const __grid_constant__ CUtensorMap tmB) {
-    using Cfg = OzCfg<KC, STAGES>;
-    constexpr int OZ_STAGES = STAGES, OZ_KC = KC;
-    constexpr int OZ_A_PLANE = Cfg::A_PLANE, OZ_B_PLANE = Cfg::B_PLANE, OZ_A_STAGE = Cfg::A_STAGE;
-    constexpr int OZ_STAGE_BYTES = Cfg::STAGE_BYTES;
-    // shared-memory matrix descriptor constants of the operand layout (see oz_default_desc):
-    //   TMODE 0: K-major SWIZZLE_64B rows of 64 B; 2: SWIZZLE_32B rows of 32 B; 1: un-swizzled interleave
-    constexpr uint32_t D_LAYOUT = TMODE == 0 ? 4u : (TMODE == 2 ? 6u : 0u);
-    constexpr uint32_t D_SBO = TMODE == 0 ? 32u : (TMODE == 2 ? 16u : 8u);
-    constexpr uint32_t D_LBO_A = TMODE == 1 ? (OZ_BM * 16 >> 4) : 1u, D_LBO_B = TMODE == 1 ? (OZ_BN * 16 >> 4) : 1u;
-    constexpr uint32_t D_KK_A = TMODE == 0 ? 2u : (TMODE == 1 ? 2u * (OZ_BM * 16 >> 4) : 0u);
-    constexpr uint32_t D_KK_B = TMODE == 0 ? 2u : (TMODE == 1 ? 2u * (OZ_BN * 16 >> 4) : 0u);
-    constexpr uint32_t D_HI = D_SBO | (1u << 14) | (D_LAYOUT << 29);
     extern __shared__ unsigned char oz_smem_raw[];
     const uint32_t raw = smem_u32(oz_smem_raw);
-    const uint32_t base = (raw + 1023u) & ~1023u;          // stage buffers: 1024-byte aligned
-    const uint32_t bars = base + OZ_STAGES * OZ_STAGE_BYTES;  // 8-byte mbarriers
-    // layout of the barrier block: full[STAGES], empty[STAGES], tfull[7], tempty[7], tmem ptr
-    const uint32_t full0 = bars, empty0 = bars + 8 * OZ_STAGES, tfull0 = bars + 16 * OZ_STAGES,
-                   tempty0 = tfull0 + 8 * OZ_S;
-    const uint32_t tmem_slot = tempty0 + 8 * OZ_S;
-    unsigned char* gen_base = oz_smem_raw + (base - raw);
-    volatile uint32_t* tmem_slot_ptr =
-        reinterpret_cast<volatile uint32_t*>(gen_base + OZ_STAGES * OZ_STAGE_BYTES + 16 * OZ_STAGES + 16 * OZ_S);
-
+    const uint32_t base = (raw + 1023u) & ~1023u;            // stage buffers: 1024-byte aligned
+    const uint32_t full0 = base + OZ_STAGES * OZ_STAGE_BYTES, empty0 = full0 + 8 * OZ_STAGES;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
     if (tid == 0) {
         for (int s = 0; s < OZ_STAGES; s++) {
             mbar_init(full0 + 8 * s, 1);
-            mbar_init(empty0 + 8 * s, 1);
-        }
-        for (int t = 0; t < OZ_S; t++) {
-            mbar_init(tfull0 + 8 * t, 1);
-            mbar_init(tempty0 + 8 * t, OZ_EPI_WARPS);
+            mbar_init(empty0 + 8 * s, OZ_MMA_WARPS);
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     }
-    if (warp == 9) {  // TMEM: all 512 columns (one CTA per SM)
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(512) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot_ptr;
+    const int64_t t_end = oz_t_end(g), t_step = oz_t_step(g);
 
-    if (warp == 8) {
+    if (warp >= OZ_MMA_WARPS) {
         // ===================== TMA producer =====================
-        if (lane == 0) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(OZ_PRODUCER_REGS));
+        if (warp == OZ_MMA_WARPS && lane == 0) {
             OzCursor cur;
             cur.init(g, oz_t_begin(g));
             uint32_t n = 0;
-            const int64_t t_end = oz_t_end(g), t_step = oz_t_step(g);
             for (; cur.t < t_end; cur.advance(g, t_step)) {
                 const OzTile tl = cur.tile(g);
-                const int rowA = tl.rowA, rowB = tl.rowB;
-                const int kch = oz_tile_kchunks<OZ_KC>(g, cur.t);
-                for (int kc = 0; kc < kch; kc++, n++) {
-                    const uint32_t st = n % OZ_STAGES, ph = (n / OZ_STAGES) & 1;
-#ifdef OZ_ABLATE_NO_TMA
-                    continue;
-#endif
-                    mbar_wait(empty0 + 8 * st, ph ^ 1);
-                    const uint32_t fb = full0 + 8 * st;
-                    mbar_expect_tx(fb, OZ_STAGE_BYTES);
-                    const uint32_t dA = base + st * OZ_STAGE_BYTES, dB = dA + OZ_A_STAGE;
-                    if (g.tma_mode != 1) {
-                        tma_load_3d(dA, &tmA, kc * OZ_KC, rowA, 0, fb);
-                        tma_load_3d(dB, &tmB, kc * OZ_KC, rowB, 0, fb);
-                    } else {
-                        tma_load_4d(dA, &tmA, 0, rowA, kc * (OZ_KC / 16), 0, fb);
-                        tma_load_4d(dB, &tmB, 0, rowB, kc * (OZ_KC / 16), 0, fb);
+                const int kch = oz_tile_kchunks(g, cur.t);
+                for (int pass = 0; pass < 2; pass++) {
+                    const int np = pass == 0 ? OZ_PASS0_GROUPS : OZ_S;   // digit planes the pass reads
+                    for (int kc = 0; kc < kch; kc++, n++) {
+                        const uint32_t st = n % OZ_STAGES, ph = (n / OZ_STAGES) & 1;
+                        mbar_wait(empty0 + 8 * st, ph ^ 1);
+                        const uint32_t fb = full0 + 8 * st;
+                        mbar_expect_tx(fb, (uint32_t)np * (OZ_A_PLANE + OZ_B_PLANE));
+                        const uint32_t dA = base + st * OZ_STAGE_BYTES, dB = dA + OZ_A_STAGE;
+                        for (int p = 0; p < np; p++) {
+                            tma_load_3d(dA + p * OZ_A_PLANE, &tmA, kc * OZ_KC, tl.rowA, p, fb);
+                            tma_load_3d(dB + p * OZ_B_PLANE, &tmB, kc * OZ_KC, tl.rowB, p, fb);
+                        }
                     }
                 }
             }
         }
-    } else if (warp == 9) {
-        // ===================== MMA issuer =====================
-        // The whole warp runs this (warp-uniform) loop so the address arithmetic stays in the uniform
-        // datapath; one elected lane issues.  Measured (round 2): with per-MMA 64-bit descriptor
-        // arithmetic in a single divergent lane the kernel was ISSUE-bound (tensor pipe 39 % active).
-        const bool leader = elect_one();
-        // instruction descriptor, kind::i8: D = S32 (2 @ [4,6)), A = B = INT8 (1 @ [7,10), [10,13)),
-        // K-major both, N >> 3 @ [17,23), M >> 4 @ [24,29)
-        constexpr uint32_t idesc = (2u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(OZ_BN >> 3) << 17) |
-                                   ((uint32_t)(OZ_BM >> 4) << 24);
-        uint32_t n = 0, it = 0;
-        const int64_t t_end = oz_t_end(g), t_step = oz_t_step(g);
-        for (int64_t t = oz_t_begin(g); t < t_end; t += t_step, it++) {
-            const int kch = oz_tile_kchunks<OZ_KC>(g, t);
-            for (int kc = 0; kc < kch; kc++, n++) {
-                const uint32_t st = n % OZ_STAGES, ph = (n / OZ_STAGES) & 1;
-#ifndef OZ_ABLATE_NO_TMA
-                mbar_wait(full0 + 8 * st, ph);
-#endif
-                tc_fence_after();
-                const uint32_t sA = base + st * OZ_STAGE_BYTES, sB = sA + OZ_A_STAGE;
-                const uint32_t a0 = (sA >> 4) | (D_LBO_A << 16), b0 = (sB >> 4) | (D_LBO_B << 16);
-                const uint32_t acc0 = kc > 0 ? 1u : 0u;
-                constexpr bool PAIRTS = PAIR && ATMEM;
-                if constexpr (PAIR && !ATMEM) {
-                    // Two digit planes of B per instruction.  Measured (round 2, tools/oz_test ablations): an
-                    // M=128 N=64 K=32 int8 MMA takes ~71 clk however its operands are fed (smem or TMEM), i.e.
-                    // the instruction has a ~64 clk floor and N=64 runs the tensor pipe at half rate.  The B
-                    // planes q and q+1 are adjacent in shared memory with the same row-group stride, so ONE
-                    // N=128 instruction computes A_p B_q^T and A_p B_{q+1}^T into the adjacent accumulators of
-                    // groups p+q and p+q+1: 16 instructions per K=32 step instead of 28.
-                    constexpr uint32_t idesc128 = (2u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(2 * OZ_BN >> 3) << 17) |
-                                                  ((uint32_t)(OZ_BM >> 4) << 24);
+        return;
+    }
+
+    // ===================== consumer warpgroups =====================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(OZ_CONSUMER_REGS));
+    const int wg = warp >> 2, wq = warp & 3;
+    // accumulator fragment of wgmma m64nN: d[j] is row 16 wq + lane/4 (+8 for j%4 >= 2), column 8 (j/4) + 2 (lane%4) + j%2
+    const int row0 = wg * 64 + wq * 16 + (lane >> 2), col0 = 2 * (lane & 3);
+    OzCursor cur;
+    cur.init(g, oz_t_begin(g));
+    uint32_t n = 0;
+    for (; cur.t < t_end; cur.advance(g, t_step)) {
+        const OzTile tl = cur.tile(g);
+        const int kch = oz_tile_kchunks(g, cur.t);
+        double acc[32];
 #pragma unroll
-                    for (int kk = 0; kk < OZ_KC / 32; kk++) {
+        for (int c = 0; c < 32; c++) acc[c] = 0.0;
+        oz_pass<0, OZ_PASS0_GROUPS>(acc, kch, n, base, full0, empty0, wg, lane);
+        oz_pass<OZ_PASS0_GROUPS, OZ_S>(acc, kch, n, base, full0, empty0, wg, lane);
+        const double si[2] = {g.scaleA[tl.rowA + row0], g.scaleA[tl.rowA + row0 + 8]};
+        if constexpr (STORE) {   // panel solve X = A W^T written straight into the packed matrix: no read of C
+            const int64_t rt = cur.t % g.mtiles, ct = cur.t / g.mtiles;
+            const int64_t ldq = g.cld[ct >> 1];
+            double* xp = g.cb[ct >> 1] + ((ct & 1) * OZ_BN) * ldq + rt * OZ_BM + row0;
 #pragma unroll
-                        for (int p = 0; p < OZ_S; p++) {
-#pragma unroll
-                            for (int q = 0; q < OZ_S - p; q += 2) {
-                                const bool two = (q + 1 < OZ_S - p);
-                                if (kc == 0 && kk == 0 && p == 0) {   // first touch of group(s) q (and q+1) in this tile
-                                    mbar_wait(tempty0 + 8 * q, (it & 1) ^ 1);
-                                    if (two) mbar_wait(tempty0 + 8 * (q + 1), (it & 1) ^ 1);
-                                    tc_fence_after();
-                                }
-                                const uint32_t alo = a0 + (uint32_t)(p * (OZ_A_PLANE >> 4)) + (uint32_t)kk * D_KK_A;
-                                const uint32_t blo = b0 + (uint32_t)(q * (OZ_B_PLANE >> 4)) + (uint32_t)kk * D_KK_B;
-                                if (leader)
-                                    mma_i8_lohi(tmem + (uint32_t)(p + q) * OZ_BN, alo, blo, D_HI, two ? idesc128 : idesc,
-                                                (p > 0 || kk > 0) ? 1u : acc0);
-                            }
-                        }
-                    }
-                    if (kc == kch - 1 && leader) {
-#pragma unroll
-                        for (int grp = 0; grp < OZ_S; grp++) tc_commit(tfull0 + 8 * grp);
-                    }
-                } else if constexpr (!ATMEM) {
-#pragma unroll
-                    for (int grp = 0; grp < OZ_S; grp++) {         // grp = p + q - 2
-                        if (kc == 0) {                              // accumulator must have been drained
-                            mbar_wait(tempty0 + 8 * grp, (it & 1) ^ 1);
-                            tc_fence_after();
-                        }
-                        const uint32_t d = tmem + (uint32_t)grp * OZ_BN;
-#pragma unroll
-                        for (int p = 0; p <= grp; p++) {            // digit planes p (of A) and q = grp - p (of B)
-                            const int q = grp - p;
-#pragma unroll
-                            for (int kk = 0; kk < OZ_KC / 32; kk++) {
-                                const uint32_t alo = a0 + (uint32_t)(p * (OZ_A_PLANE >> 4)) + (uint32_t)kk * D_KK_A;
-                                const uint32_t blo = b0 + (uint32_t)(q * (OZ_B_PLANE >> 4)) + (uint32_t)kk * D_KK_B;
-#ifndef OZ_ABLATE_NO_MMA
-                                if (leader) mma_i8_lohi(d, alo, blo, D_HI, idesc, (p > 0 || kk > 0) ? 1u : acc0);
-#endif
-                            }
-                        }
-                        if (kc == kch - 1 && leader) tc_commit(tfull0 + 8 * grp);   // G_{grp+2} of this tile is final
-                    }
-                } else {
-                    // A operand through TMEM: the 7 digit planes of one K = 32 step are copied smem -> TMEM
-                    // once (tcgen05.cp, 8 columns each, columns 448..503) and every MMA of the step then
-                    // reads only B from shared memory: 2 KB instead of 6 KB per MMA.  In SS mode the kernel
-                    // is shared-memory-bandwidth bound (ncu: 83 % of the smem pipe, 72 clk per N=64 MMA whose
-                    // tensor floor is 32 clk).  tcgen05.cp and tcgen05.mma execute in issue order, so the
-                    // next step's copies cannot overtake the MMAs still reading the slab.
-                    constexpr uint32_t A_TMEM_COL = OZ_S * OZ_BN;   // 448
-#pragma unroll
-                    for (int kk = 0; kk < OZ_KC / 32; kk++) {
-#pragma unroll
-                        for (int p = 0; p < OZ_S; p++) {
-                            const uint32_t alo = a0 + (uint32_t)(p * (OZ_A_PLANE >> 4)) + (uint32_t)kk * D_KK_A;
-                            if (leader) tmem_cp_128x256b(tmem + A_TMEM_COL + (uint32_t)p * 8, alo, D_HI);
-                        }
-                        if constexpr (!PAIRTS) {
-#pragma unroll
-                            for (int grp = 0; grp < OZ_S; grp++) {
-                                if (kc == 0 && kk == 0) {
-                                    mbar_wait(tempty0 + 8 * grp, (it & 1) ^ 1);
-                                    tc_fence_after();
-                                }
-                                const uint32_t d = tmem + (uint32_t)grp * OZ_BN;
-#pragma unroll
-                                for (int p = 0; p <= grp; p++) {
-                                    const int q = grp - p;
-                                    const uint32_t blo = b0 + (uint32_t)(q * (OZ_B_PLANE >> 4)) + (uint32_t)kk * D_KK_B;
-                                    if (leader)
-                                        mma_i8_ts(d, tmem + A_TMEM_COL + (uint32_t)p * 8, blo, D_HI, idesc,
-                                                  (p > 0 || kk > 0) ? 1u : acc0);
-                                }
-                                if (kc == kch - 1 && kk == OZ_KC / 32 - 1 && leader) tc_commit(tfull0 + 8 * grp);
-                            }
-                        } else {
-                            // A from TMEM AND two B planes per instruction (N = 128)
-                            constexpr uint32_t idesc128 = (2u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(2 * OZ_BN >> 3) << 17) |
-                                                          ((uint32_t)(OZ_BM >> 4) << 24);
-#pragma unroll
-                            for (int p = 0; p < OZ_S; p++) {
-#pragma unroll
-                                for (int q = 0; q < OZ_S - p; q += 2) {
-                                    const bool two = (q + 1 < OZ_S - p);
-                                    if (kc == 0 && kk == 0 && p == 0) {
-                                        mbar_wait(tempty0 + 8 * q, (it & 1) ^ 1);
-                                        if (two) mbar_wait(tempty0 + 8 * (q + 1), (it & 1) ^ 1);
-                                        tc_fence_after();
-                                    }
-                                    const uint32_t blo = b0 + (uint32_t)(q * (OZ_B_PLANE >> 4)) + (uint32_t)kk * D_KK_B;
-                                    if (leader)
-                                        mma_i8_ts(tmem + (uint32_t)(p + q) * OZ_BN, tmem + A_TMEM_COL + (uint32_t)p * 8, blo, D_HI,
-                                                  two ? idesc128 : idesc, (p > 0 || kk > 0) ? 1u : acc0);
-                                }
-                            }
-                            if (kc == kch - 1 && kk == OZ_KC / 32 - 1 && leader) {
-#pragma unroll
-                                for (int grp = 0; grp < OZ_S; grp++) tc_commit(tfull0 + 8 * grp);
-                            }
-                        }
-                    }
-                }
-#ifndef OZ_ABLATE_NO_TMA
-                if (leader) tc_commit(empty0 + 8 * st);  // smem stage free once these MMAs have read it
-#endif
-                __syncwarp();
+            for (int j = 0; j < 32; j++) {
+                const int r = (j & 2) ? 8 : 0, c = 8 * (j >> 2) + col0 + (j & 1);
+                xp[(int64_t)c * ldq + r] = (si[r >> 3] * g.scaleB[tl.rowB + c]) * acc[j];
             }
-        }
-    } else {
-        // ===================== epilogue warps 0..7 =====================
-        oz_epilogue<STORE>(g, tmem, tfull0, tempty0, warp, lane);
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 9) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512) : "memory");
-    }
-}
-
-// ---- ring-pipelined variant (the one that ships) ---------------------------------------------------
-// Measured on B200 (tools/mb_tcgen05, tools/oz_test ablations, profiles/): an M=128 N=64 K=32 int8 MMA
-// with both operands in shared memory takes 48 clk (smem-bound: 6 KB of operands per instruction), N=128
-// takes 64 clk = the 4.57 POP/s peak; the TMA path delivers ~80 GB/s per SM (8.6 us for the 688 KB of a
-// tile) with ~2 us latency, so the 2 x 84 KB stage ring above can keep at most ONE stage in flight and the
-// MMA and TMA times ADD (15.8 us per tile instead of max(7.8, 8.6)).  Here the ring is fine-grained:
-//   * B (7 planes x 64 rows x 64 B = 28 KB per k-chunk) is double-buffered,
-//   * A streams plane by plane (128 rows x 64 B = 8 KB) through a deep ring of RING_A slots, each with
-//     its own full/empty mbarrier: the MMA warp consumes plane p while planes p+1.. of this and the next
-//     k-chunks are still landing -- ~170 KB in flight instead of 84 KB,
-//   * MMAs are issued per A plane against PAIRS of adjacent B planes (N = 128: two accumulators at once).
-constexpr int RING_A = 18;           // A-plane slots of 8 KB
-constexpr int RING_B = 2;            // B stages of 28 KB
-constexpr int RK = 64;               // bytes of K per chunk (SWIZZLE_64B rows)
-constexpr int RA_SLOT = OZ_BM * RK;  // 8192
-constexpr int RB_PLANE = OZ_BN * RK; // 4096
-constexpr int RB_STAGE = OZ_S * RB_PLANE;  // 28672
-constexpr size_t RING_SMEM = (size_t)RING_B * RB_STAGE + (size_t)RING_A * RA_SLOT + 1024 + 8 * (2 * RING_A + 2 * RING_B + 2 * OZ_S) + 64;
-
-__global__ void __launch_bounds__(OZ_THREADS, 1)
-ozaki_ring_kernel(const __grid_constant__ OzArgs g, const __grid_constant__ CUtensorMap tmA1,
-                  const __grid_constant__ CUtensorMap tmB) {
-    constexpr uint32_t D_HI = 32u | (1u << 14) | (4u << 29);   // SBO 512 B, version 1, SWIZZLE_64B
-    extern __shared__ unsigned char oz_smem_raw[];
-    const uint32_t raw = smem_u32(oz_smem_raw);
-    const uint32_t base = (raw + 1023u) & ~1023u;
-    const uint32_t sB0 = base, sA0 = base + RING_B * RB_STAGE;
-    const uint32_t bars = sA0 + RING_A * RA_SLOT;
-    const uint32_t fullA = bars, emptyA = fullA + 8 * RING_A, fullB = emptyA + 8 * RING_A, emptyB = fullB + 8 * RING_B,
-                   tfull0 = emptyB + 8 * RING_B, tempty0 = tfull0 + 8 * OZ_S, tmem_slot = tempty0 + 8 * OZ_S;
-    volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(oz_smem_raw + (tmem_slot - raw));
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-
-    if (tid == 0) {
-        for (int i = 0; i < RING_A; i++) { mbar_init(fullA + 8 * i, 1); mbar_init(emptyA + 8 * i, 1); }
-        for (int i = 0; i < RING_B; i++) { mbar_init(fullB + 8 * i, 1); mbar_init(emptyB + 8 * i, 1); }
-        for (int t = 0; t < OZ_S; t++) { mbar_init(tfull0 + 8 * t, 1); mbar_init(tempty0 + 8 * t, OZ_EPI_WARPS); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    }
-    if (warp == 9) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(512) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot_ptr;
-
-    if (warp == 8) {
-        // ===================== TMA producer =====================
-        if (lane == 0) {
-            OzCursor cur;
-            cur.init(g, oz_t_begin(g));
-            uint32_t na = 0, nb = 0;
-            const int64_t t_end = oz_t_end(g), t_step = oz_t_step(g);
-            for (; cur.t < t_end; cur.advance(g, t_step)) {
-                const OzTile tl = cur.tile(g);
-                const int kch = oz_tile_kchunks<RK>(g, cur.t);
-                for (int kc = 0; kc < kch; kc++, nb++) {
-                    {
-                        const uint32_t bs = nb % RING_B, ph = (nb / RING_B) & 1;
-                        mbar_wait(emptyB + 8 * bs, ph ^ 1);
-                        mbar_expect_tx(fullB + 8 * bs, RB_STAGE);
-                        tma_load_3d(sB0 + bs * RB_STAGE, &tmB, kc * RK, tl.rowB, 0, fullB + 8 * bs);
-                    }
-#pragma unroll 1
-                    for (int p = 0; p < OZ_S; p++, na++) {
-                        const uint32_t sl = na % RING_A, ph = (na / RING_A) & 1;
-                        mbar_wait(emptyA + 8 * sl, ph ^ 1);
-                        mbar_expect_tx(fullA + 8 * sl, RA_SLOT);
-                        tma_load_3d(sA0 + sl * RA_SLOT, &tmA1, kc * RK, tl.rowA, p, fullA + 8 * sl);
-                    }
+        } else {
+            double* cp = tl.C + row0;
+            const int64_t ldc = tl.ldc;
+#pragma unroll
+            for (int j0 = 0; j0 < 32; j0 += 8) {
+                double old[8];
+#pragma unroll
+                for (int j = j0; j < j0 + 8; j++) {
+                    const int r = (j & 2) ? 8 : 0, c = 8 * (j >> 2) + col0 + (j & 1);
+                    old[j - j0] = __ldcs(cp + (int64_t)c * ldc + r);
+                }
+#pragma unroll
+                for (int j = j0; j < j0 + 8; j++) {
+                    const int r = (j & 2) ? 8 : 0, c = 8 * (j >> 2) + col0 + (j & 1);
+                    cp[(int64_t)c * ldc + r] = fma(-(si[r >> 3] * g.scaleB[tl.rowB + c]), acc[j], old[j - j0]);
                 }
             }
         }
-    } else if (warp == 9) {
-        // ===================== MMA issuer (whole warp runs the loop, one elected lane issues) ==========
-        const bool leader = elect_one();
-        constexpr uint32_t idesc64 = (2u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(OZ_BN >> 3) << 17) | ((uint32_t)(OZ_BM >> 4) << 24);
-        constexpr uint32_t idesc128 = (2u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(2 * OZ_BN >> 3) << 17) | ((uint32_t)(OZ_BM >> 4) << 24);
-        uint32_t na = 0, nb = 0, it = 0;
-        const int64_t t_end = oz_t_end(g), t_step = oz_t_step(g);
-        for (int64_t t = oz_t_begin(g); t < t_end; t += t_step, it++) {
-            const int kch = oz_tile_kchunks<RK>(g, t);
-            for (int kc = 0; kc < kch; kc++, nb++) {
-                const uint32_t bs = nb % RING_B;
-                mbar_wait(fullB + 8 * bs, (nb / RING_B) & 1);
-                const uint32_t b0 = ((sB0 + bs * RB_STAGE) >> 4) | (1u << 16);
-                const uint32_t acc0 = kc > 0 ? 1u : 0u;
-#pragma unroll
-                for (int p = 0; p < OZ_S; p++, na++) {
-                    const uint32_t sl = na % RING_A;
-                    mbar_wait(fullA + 8 * sl, (na / RING_A) & 1);
-                    tc_fence_after();
-                    const uint32_t a0 = ((sA0 + sl * RA_SLOT) >> 4) | (1u << 16);
-#pragma unroll
-                    for (int kk = 0; kk < RK / 32; kk++) {
-#pragma unroll
-                        for (int q = 0; q < OZ_S - p; q += 2) {
-                            const bool two = (q + 1 < OZ_S - p);
-                            if (kc == 0 && kk == 0 && p == 0) {   // first touch of group(s) q (and q+1) in this tile
-                                mbar_wait(tempty0 + 8 * q, (it & 1) ^ 1);
-                                if (two) mbar_wait(tempty0 + 8 * (q + 1), (it & 1) ^ 1);
-                                tc_fence_after();
-                            }
-                            if (leader)
-                                mma_i8_lohi(tmem + (uint32_t)(p + q) * OZ_BN, a0 + (uint32_t)kk * 2u,
-                                            b0 + (uint32_t)(q * (RB_PLANE >> 4)) + (uint32_t)kk * 2u, D_HI,
-                                            two ? idesc128 : idesc64, (p > 0 || kk > 0) ? 1u : acc0);
-                        }
-                    }
-                    if (leader) tc_commit(emptyA + 8 * sl);     // A plane slot free once these MMAs have read it
-                }
-                if (leader) tc_commit(emptyB + 8 * bs);
-                if (kc == kch - 1 && leader) {
-#pragma unroll
-                    for (int grp = 0; grp < OZ_S; grp++) tc_commit(tfull0 + 8 * grp);
-                }
-                __syncwarp();
-            }
-        }
-    } else {
-        oz_epilogue<false>(g, tmem, tfull0, tempty0, warp, lane);
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 9) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512) : "memory");
     }
 }
 
@@ -783,16 +402,6 @@ EncodeTiled_t g_encode = nullptr;
 bool g_oz_attr = false;
 int g_oz_sms = 0;
 
-// tma_mode -> (KC, STAGES) instance
-#define OZ_DISPATCH(mode, CALL)                                  \
-    do {                                                         \
-        if ((mode) == 2) { CALL(32, 5, 2, false, false); } else if ((mode) == 1) { CALL(64, 2, 1, false, false); }       \
-        else if ((mode) == 4) { CALL(64, 2, 0, true, false); } else if ((mode) == 6) { CALL(32, 5, 2, true, false); }     \
-        else if ((mode) == 8) { CALL(64, 2, 0, false, true); } else if ((mode) == 10) { CALL(32, 5, 2, false, true); }    \
-        else if ((mode) == 12) { CALL(64, 2, 0, true, true); }                                                            \
-        else { CALL(64, 2, 0, false, false); }                                                                            \
-    } while (0)
-
 int oz_init() {
     if (!g_encode) {
         void* fn = nullptr;
@@ -801,16 +410,9 @@ int oz_init() {
         g_encode = (EncodeTiled_t)fn;
     }
     if (!g_oz_attr) {
-#define OZ_ATTR(KC, ST, TM, AT, PR)                                                                              \
-        if (cudaFuncSetAttribute(ozaki_syrk_kernel<KC, ST, TM, AT, PR>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
-                                 (int)OzCfg<KC, ST>::SMEM) != cudaSuccess) return -2
-        OZ_ATTR(64, 2, 0, false, false); OZ_ATTR(64, 2, 1, false, false); OZ_ATTR(32, 5, 2, false, false);
-        OZ_ATTR(64, 2, 0, true, false); OZ_ATTR(32, 5, 2, true, false);
-        OZ_ATTR(64, 2, 0, false, true); OZ_ATTR(32, 5, 2, false, true); OZ_ATTR(64, 2, 0, true, true);
-        if (cudaFuncSetAttribute(ozaki_syrk_kernel<64, 2, 0, false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 (int)OzCfg<64, 2>::SMEM) != cudaSuccess) return -2;
-        if (cudaFuncSetAttribute(ozaki_ring_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RING_SMEM) != cudaSuccess) return -2;
-#undef OZ_ATTR
+        if (cudaFuncSetAttribute(ozaki_syrk_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)OZ_SMEM) != cudaSuccess ||
+            cudaFuncSetAttribute(ozaki_syrk_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)OZ_SMEM) != cudaSuccess)
+            return -2;
         int dev = 0;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&g_oz_sms, cudaDevAttrMultiProcessorCount, dev);
@@ -823,50 +425,21 @@ int oz_init() {
 
 size_t oz_planes_bytes(int64_t Np) { return (size_t)OZ_S * Np * OZ_KMAX; }
 
-// Build the two tensor maps (A box: 128 rows, B box: 64 rows) over the digit planes.
-int oz_make_maps(signed char* planes, int64_t Np, int tma_mode, OzMaps* out) {
+// The two tensor maps over the digit planes: one plane of a 64-byte k-chunk of 128 rows (A) / 64 rows (B)
+// per copy, SWIZZLE_64B.
+int oz_make_maps(signed char* planes, int64_t Np, OzMaps* out) {
     if (oz_init() != 0) return -1;
-    tma_mode = tma_mode >= 16 ? 0 : (tma_mode & 3);   // bits 2 / 3 / 4 only select kernel variants (A via TMEM / paired N / ring)
     static_assert(sizeof(out->a) >= sizeof(CUtensorMap), "OzMaps too small");
-    CUtensorMap* ma = reinterpret_cast<CUtensorMap*>(out->a);
-    CUtensorMap* mb = reinterpret_cast<CUtensorMap*>(out->b);
-    CUresult r1, r2;
-    {   // single-plane A box of the ring kernel (always built: 128 rows x 64 B x 1 plane, SWIZZLE_64B)
-        CUtensorMap* m1 = reinterpret_cast<CUtensorMap*>(out->a1);
-        cuuint64_t dims[3] = {(cuuint64_t)OZ_KMAX, (cuuint64_t)Np, (cuuint64_t)OZ_S};
-        cuuint64_t strides[2] = {(cuuint64_t)OZ_KMAX, (cuuint64_t)Np * OZ_KMAX};
-        cuuint32_t estr[3] = {1, 1, 1};
-        cuuint32_t box1[3] = {64, OZ_BM, 1};
-        if (g_encode(m1, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, planes, dims, strides, box1, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-            return -3;
-    }
-    if (tma_mode == 0 || tma_mode == 2) {
-        const cuuint32_t kc = tma_mode == 0 ? 64 : 32;
-        const CUtensorMapSwizzle sw = tma_mode == 0 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B;
-        cuuint64_t dims[3] = {(cuuint64_t)OZ_KMAX, (cuuint64_t)Np, (cuuint64_t)OZ_S};
-        cuuint64_t strides[2] = {(cuuint64_t)OZ_KMAX, (cuuint64_t)Np * OZ_KMAX};
-        cuuint32_t estr[3] = {1, 1, 1};
-        cuuint32_t boxA[3] = {kc, OZ_BM, OZ_S}, boxB[3] = {kc, OZ_BN, OZ_S};
-        r1 = g_encode(ma, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, planes, dims, strides, boxA, estr,
-                      CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        r2 = g_encode(mb, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, planes, dims, strides, boxB, estr,
-                      CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    } else {
-        // un-swizzled "interleave" operand layout: smem [plane][16-byte k column][row][16 B]
-        cuuint64_t dims[4] = {16, (cuuint64_t)Np, (cuuint64_t)(OZ_KMAX / 16), (cuuint64_t)OZ_S};
-        cuuint64_t strides[3] = {(cuuint64_t)OZ_KMAX, 16, (cuuint64_t)Np * OZ_KMAX};
-        cuuint32_t estr[4] = {1, 1, 1, 1};
-        cuuint32_t boxA[4] = {16, OZ_BM, 64 / 16, OZ_S}, boxB[4] = {16, OZ_BN, 64 / 16, OZ_S};
-        r1 = g_encode(ma, CU_TENSOR_MAP_DATA_TYPE_UINT8, 4, planes, dims, strides, boxA, estr,
-                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        r2 = g_encode(mb, CU_TENSOR_MAP_DATA_TYPE_UINT8, 4, planes, dims, strides, boxB, estr,
-                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    }
+    cuuint64_t dims[3] = {(cuuint64_t)OZ_KMAX, (cuuint64_t)Np, (cuuint64_t)OZ_S};
+    cuuint64_t strides[2] = {(cuuint64_t)OZ_KMAX, (cuuint64_t)Np * OZ_KMAX};
+    cuuint32_t estr[3] = {1, 1, 1};
+    cuuint32_t boxA[3] = {OZ_KC, OZ_BM, 1}, boxB[3] = {OZ_KC, OZ_BN, 1};
+    const CUresult r1 = g_encode(reinterpret_cast<CUtensorMap*>(out->a), CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, planes, dims,
+                                 strides, boxA, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B,
+                                 CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    const CUresult r2 = g_encode(reinterpret_cast<CUtensorMap*>(out->b), CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, planes, dims,
+                                 strides, boxB, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B,
+                                 CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     return (r1 == CUDA_SUCCESS && r2 == CUDA_SUCCESS) ? 0 : -3;
 }
 
@@ -888,36 +461,7 @@ OzSrc oz_src_tiled(const double* const* Pt, int nseg) {
     return src;
 }
 
-void oz_default_desc(OzDesc* d, int tma_mode) {
-    tma_mode = tma_mode >= 16 ? 0 : (tma_mode & 3);
-    if (tma_mode == 0) {
-        d->a_kk_adv = d->b_kk_adv = 2;  // +32 bytes inside the 64-byte swizzled row
-        d->a_lbo = d->b_lbo = 1;        // unused for swizzled K-major
-        d->sbo = 32;                    // 8 rows x 64 B
-        d->layout = 4;                  // SWIZZLE_64B
-    } else if (tma_mode == 2) {
-        d->a_kk_adv = d->b_kk_adv = 0;  // one K=32 step per stage
-        d->a_lbo = d->b_lbo = 1;
-        d->sbo = 16;                    // 8 rows x 32 B
-        d->layout = 6;                  // SWIZZLE_32B
-    } else {
-        d->a_kk_adv = 2 * (OZ_BM * 16 >> 4);  // two 16-byte k columns of 128 rows
-        d->b_kk_adv = 2 * (OZ_BN * 16 >> 4);
-        d->a_lbo = OZ_BM * 16 >> 4;           // next 16-byte k column
-        d->b_lbo = OZ_BN * 16 >> 4;
-        d->sbo = 8;                           // next 8-row core matrix: 128 B
-        d->layout = 0;
-    }
-}
-
-static void oz_fill_desc(OzArgs& g, const OzDesc* desc, int tma_mode, int* dbg) {
-    g.a_kk_adv = desc->a_kk_adv; g.b_kk_adv = desc->b_kk_adv;
-    g.a_lbo = desc->a_lbo; g.b_lbo = desc->b_lbo; g.sbo = desc->sbo; g.layout = desc->layout;
-    g.tma_mode = tma_mode;
-    g.dbg = dbg;
-}
-
-static int oz_launch(OzArgs& g, const OzMaps* mapsA, const OzMaps* mapsB, cudaStream_t s, int reserve_sms) {
+static int oz_launch(OzArgs& g, const OzMaps* mapsA, const OzMaps* mapsB, bool store, cudaStream_t s, int reserve_sms) {
     int64_t cap = g_oz_sms - reserve_sms;
     if (cap < 1) cap = 1;
     if (g.tile_hi <= 0 || g.tile_hi > g.total_tiles) g.tile_hi = g.total_tiles;
@@ -931,20 +475,8 @@ static int oz_launch(OzArgs& g, const OzMaps* mapsA, const OzMaps* mapsB, cudaSt
     }
     const CUtensorMap* ma = reinterpret_cast<const CUtensorMap*>(mapsA->a);
     const CUtensorMap* mb = reinterpret_cast<const CUtensorMap*>(mapsB->b);
-    if (g.tma_mode >= 16) {
-        const CUtensorMap* m1 = reinterpret_cast<const CUtensorMap*>(mapsA->a1);
-        ozaki_ring_kernel<<<(unsigned)grid, OZ_THREADS, RING_SMEM, s>>>(g, *m1, *mb);
-        g_launch_count++;
-        return 0;
-    }
-    if (g.store) {   // panel solve: one instance only (SWIZZLE_64B maps, paired N)
-        ozaki_syrk_kernel<64, 2, 0, false, true, true><<<(unsigned)grid, OZ_THREADS, OzCfg<64, 2>::SMEM, s>>>(g, *ma, *mb);
-        g_launch_count++;
-        return 0;
-    }
-#define OZ_LAUNCH(KC, ST, TM, AT, PR) ozaki_syrk_kernel<KC, ST, TM, AT, PR><<<(unsigned)grid, OZ_THREADS, OzCfg<KC, ST>::SMEM, s>>>(g, *ma, *mb)
-    OZ_DISPATCH(g.tma_mode, OZ_LAUNCH);
-#undef OZ_LAUNCH
+    if (store) ozaki_syrk_kernel<true><<<(unsigned)grid, OZ_THREADS, OZ_SMEM, s>>>(g, *ma, *mb);
+    else ozaki_syrk_kernel<false><<<(unsigned)grid, OZ_THREADS, OZ_SMEM, s>>>(g, *ma, *mb);
     g_launch_count++;
     return 0;
 }
@@ -952,8 +484,8 @@ static int oz_launch(OzArgs& g, const OzMaps* mapsA, const OzMaps* mapsB, cudaSt
 // A[I, J] -= P_I P_J^T on the packed lower matrix for the owned block columns J in [jlo, jhi), with
 // the digit planes / scales produced by launch_oz_slice.  K = 128 * nseg.
 int launch_syrk_ozaki(Packed Apk, int64_t k, int nseg, int64_t jlo, int64_t jhi, int rank, int world,
-                      const OzMaps* maps, const double* scale, const OzDesc* desc, int tma_mode, cudaStream_t s,
-                      int reserve_sms, int* dbg, int64_t tile_lo, int64_t tile_hi) {
+                      const OzMaps* maps, const double* scale, cudaStream_t s, int reserve_sms, int64_t tile_lo,
+                      int64_t tile_hi) {
     if (oz_init() != 0) return -1;
     const int64_t nblk = Apk.nblk();
     if (jlo < k + 1) jlo = k + 1;
@@ -966,10 +498,9 @@ int launch_syrk_ozaki(Packed Apk, int64_t k, int nseg, int64_t jlo, int64_t jhi,
     g.Pk = Apk; g.J0 = J0; g.w = world;
     g.total_tiles = tiles * 2;
     g.tile_lo = tile_lo; g.tile_hi = tile_hi;   // (0, 0): everything
-    g.kchunks = nseg * NB / ((tma_mode < 16 && (tma_mode & 3) == 2) ? 32 : 64);
+    g.kchunks = nseg * NB / OZ_KC;
     g.scaleA = g.scaleB = scale;
-    oz_fill_desc(g, desc, tma_mode, dbg);
-    return oz_launch(g, maps, maps, s, reserve_sms);
+    return oz_launch(g, maps, maps, false, s, reserve_sms);
 }
 
 // plain product  C[M x Ncols] -= A B^T  (C dense column-major, ldc; M % 128 == 0, Ncols % 64 == 0):
@@ -977,7 +508,7 @@ int launch_syrk_ozaki(Packed Apk, int64_t k, int nseg, int64_t jlo, int64_t jhi,
 // (mapsB, scaleB); K = 128 * nseg.  Used by the posterior / VFE matrix-TRSM sweeps.
 int launch_gemm_ozaki(double* C, int64_t ldc, int64_t M, int64_t Ncols, int nseg, const OzMaps* mapsA,
                       const double* scaleA, int64_t rowA0, const OzMaps* mapsB, const double* scaleB, int64_t rowB0,
-                      const OzDesc* desc, int tma_mode, cudaStream_t s) {
+                      cudaStream_t s) {
     if (oz_init() != 0) return -1;
     if (M <= 0 || Ncols <= 0 || nseg <= 0) return 0;
     OzArgs g{};
@@ -986,33 +517,30 @@ int launch_gemm_ozaki(double* C, int64_t ldc, int64_t M, int64_t Ncols, int nseg
     g.c_rt_stride = OZ_BM;
     g.c_pair_stride = 2 * OZ_BN * ldc;
     g.total_tiles = (M / OZ_BM) * (Ncols / OZ_BN);
-    g.kchunks = nseg * NB / ((tma_mode < 16 && (tma_mode & 3) == 2) ? 32 : 64);
+    g.kchunks = nseg * NB / OZ_KC;
     g.scaleA = scaleA; g.scaleB = scaleB;
     g.rowA0 = rowA0; g.rowB0 = rowB0;
-    oz_fill_desc(g, desc, tma_mode, nullptr);
-    return oz_launch(g, mapsA, mapsB, s, 0);
+    return oz_launch(g, mapsA, mapsB, false, s, 0);
 }
 
 // Panel solve of the wide panel phase:  X[M x 512] = A W^T, W = inv(L_512) block lower triangular (K blocks above
 // the diagonal are skipped), written over the four block columns Xcol[q] (leading dimensions ldx[q]) the planes of A
-// were cut from.  Needs SWIZZLE_64B maps (tma_mode & 3 == 0).
+// were cut from.
 int launch_panel_solve_ozaki(double* const* Xcol, const int64_t* ldx, int64_t M, const OzMaps* mapsA, const double* scaleA,
-                             int64_t rowA0, const OzMaps* mapsW, const double* scaleW, const OzDesc* desc, cudaStream_t s) {
+                             int64_t rowA0, const OzMaps* mapsW, const double* scaleW, cudaStream_t s) {
     if (oz_init() != 0) return -1;
     if (M <= 0) return 0;
     OzArgs g{};
     g.mode = 0;
     g.mtiles = M / OZ_BM;
     g.total_tiles = (M / OZ_BM) * (4 * NB / OZ_BN);
-    g.kchunks = 4 * NB / 64;
+    g.kchunks = 4 * NB / OZ_KC;
     g.tri = 1;
-    g.store = 1;
     for (int q = 0; q < 4; q++) { g.cb[q] = Xcol[q]; g.cld[q] = ldx[q]; }
     g.C = Xcol[0]; g.ldc = ldx[0]; g.c_rt_stride = OZ_BM; g.c_pair_stride = 0;
     g.scaleA = scaleA; g.scaleB = scaleW;
     g.rowA0 = rowA0; g.rowB0 = 0;
-    oz_fill_desc(g, desc, 8, nullptr);
-    return oz_launch(g, mapsA, mapsW, s, 0);
+    return oz_launch(g, mapsA, mapsW, true, s, 0);
 }
 
 }  // namespace sb

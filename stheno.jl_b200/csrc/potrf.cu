@@ -102,7 +102,7 @@ potrf_inv_kernel(Packed A, int64_t k, int64_t N, double* __restrict__ invL,
 #pragma unroll
             for (int p = 0; p < PB; p++) li[p] = s[(j0 + p) * LDS + ri];
             // two columns per iteration: two independent FMA chains (the 8-deep dependent chain was
-            // latency-bound: potrf_inv measured 198 us per block in round 1, all of the panel chain)
+            // latency-bound, and potrf_inv is the serial panel chain)
             int l = j0 + PB + lg;
             for (; l + PT / NB <= ri; l += 2 * (PT / NB)) {
                 const int l2 = l + PT / NB;

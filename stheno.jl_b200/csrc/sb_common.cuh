@@ -1,4 +1,4 @@
-// Shared definitions for libstheno_b200 (sm_100a only).
+// Shared definitions for libstheno_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -173,12 +173,10 @@ void launch_pack_lower(Packed L, const double* D, int64_t ld, double shift, cuda
 void launch_add_diag(Packed L, const double* d, int64_t n, cudaStream_t st);
 void launch_add_dense_lower(Packed L, const double* D, int64_t ld, int64_t n, cudaStream_t st);
 
-// ---- K3': trailing update on tcgen05 (int8 Ozaki slicing), ozaki.cu ------------------------------
-struct alignas(64) OzMaps { unsigned char a[128]; unsigned char b[128]; unsigned char a1[128]; };  // CUtensorMap blobs: A box, B box, single-plane A box
-struct OzDesc { uint32_t a_kk_adv, b_kk_adv, a_lbo, b_lbo, sbo, layout; };
+// ---- K3': trailing update on the int8 tensor cores (wgmma, int8 Ozaki slicing), ozaki.cu ------------------
+struct alignas(64) OzMaps { unsigned char a[128]; unsigned char b[128]; };  // CUtensorMap blobs: A box (128 rows), B box (64 rows)
 size_t oz_planes_bytes(int64_t Np);                       // 7 digit planes, 512-byte row pitch
-int oz_make_maps(signed char* planes, int64_t Np, int tma_mode, OzMaps* out);
-void oz_default_desc(OzDesc* d, int tma_mode);
+int oz_make_maps(signed char* planes, int64_t Np, OzMaps* out);
 // source panel of the slicer: up to 4 segments of 128 columns; element (row block rb, col k, row r) of
 // segment q at base[q] + rb*rbs[q] + k*ld[q] + r
 struct OzSrc { const double* base[4]; int64_t ld[4]; int64_t rbs[4]; int nseg; };
@@ -186,16 +184,16 @@ OzSrc oz_src_tiled(const double* const* Pt, int nseg);
 void launch_oz_slice(const OzSrc& src, int64_t rb_lo, int64_t nrb, int64_t out_row_base, int64_t plane_rows,
                      double* scale, int* expo, signed char* planes, cudaStream_t s);
 int launch_syrk_ozaki(Packed A, int64_t k, int nseg, int64_t jlo, int64_t jhi, int rank, int world,
-                      const OzMaps* maps, const double* scale, const OzDesc* desc, int tma_mode, cudaStream_t s,
-                      int reserve_sms = 0, int* dbg = nullptr, int64_t tile_lo = 0, int64_t tile_hi = 0);
+                      const OzMaps* maps, const double* scale, cudaStream_t s, int reserve_sms = 0,
+                      int64_t tile_lo = 0, int64_t tile_hi = 0);
 
 // plain product C[M x Ncols] -= A B^T through the same kernel (dense column-major C)
 int launch_gemm_ozaki(double* C, int64_t ldc, int64_t M, int64_t Ncols, int nseg, const OzMaps* mapsA,
                       const double* scaleA, int64_t rowA0, const OzMaps* mapsB, const double* scaleB, int64_t rowB0,
-                      const OzDesc* desc, int tma_mode, cudaStream_t s);
+                      cudaStream_t s);
 // X = A inv(L_512)^T over four block columns of the packed matrix (wide panel phase, ozaki.cu)
 int launch_panel_solve_ozaki(double* const* Xcol, const int64_t* ldx, int64_t M, const OzMaps* mapsA, const double* scaleA,
-                             int64_t rowA0, const OzMaps* mapsW, const double* scaleW, const OzDesc* desc, cudaStream_t s);
+                             int64_t rowA0, const OzMaps* mapsW, const double* scaleW, cudaStream_t s);
 
 extern thread_local int64_t g_launch_count;
 

@@ -106,7 +106,7 @@ gemvT_below_kernel(Packed L, int64_t k, double* __restrict__ b, int S) {
 
 // ---- persistent triangular sweep ------------------------------------------------------------
 // One launch per sweep instead of 2 launches per 128-wide block (1024 tiny dependent launches at
-// N = 65536, 0.2 of the HBM roofline in round 1).  Right-looking data flow with static ownership:
+// N = 65536 would leave the sweep launch-latency bound).  Right-looking data flow with static ownership:
 //   forward  b <- L^{-1} b :  when x_k = invL_kk b_k is final, every block row i > k applies
 //                             b_i -= L[i,k] x_k;  b_{k+1} is final after k+1 such updates.
 //   backward b <- L^{-T} b :  when x_k = invL_kk^T b_k is final, every block j < k applies
@@ -218,8 +218,8 @@ __device__ __forceinline__ void block_matvec_t(const double* __restrict__ M, int
 }
 
 __device__ __forceinline__ void prefetch_block_l2(const double* M, int64_t ld);
-// variant A: dedicated CTA for the diagonal solves, done[] counters (round-2 measurement: 12-15 ms per
-// sweep at N = 65536; variant B below -- owner does the diagonal solve, L2 prefetch -- measured 23-34 ms)
+// variant A: dedicated CTA for the diagonal solves, done[] counters; variant B below -- owner does the
+// diagonal solve, L2 prefetch -- is the alternative (sweep_variant)
 template <bool BACKWARD, bool PF>
 __global__ void __launch_bounds__(256) sweep_kernel_a(SweepArgs a) {
     __shared__ double xs[MAXS][NB];
@@ -366,7 +366,7 @@ __global__ void __launch_bounds__(256) sweep_kernel_b(SweepArgs a) {
     }
 }
 
-// Deterministic reductions (round 2): per-block partial sums land in a scratch buffer and are added in
+// Deterministic reductions: per-block partial sums land in a scratch buffer and are added in
 // a fixed order by a second tiny kernel -- no fp64 atomics, so logpdf / mean / var are bit-reproducible
 // from run to run (and an imported factor reproduces the original bit for bit).
 __global__ void __launch_bounds__(256)

@@ -1,8 +1,8 @@
-"""FiniteGP-level API on the B200 path: logpdf / posterior / marginals / rand / elbo.
+"""FiniteGP-level API on the CUDA path: logpdf / posterior / marginals / rand / elbo.
 
 Mirror of the AbstractGPs entry points the reference reaches through Stheno
 (`logpdf(f(x, s), y)`, `posterior`, `mean/cov/var/marginals`, `rand`, `elbo(VFE(fz), fx, y)`;
-call sites /root/reference/README.md:61-96, src/gp/sparse_finite_gp.jl:52-62,
+call sites Stheno.jl README.md:61-96, src/gp/sparse_finite_gp.jl:52-62,
 test/gp/util.jl:9-88).  The interception is one level above the reference's seam
 (docs/src/internals.md:8-24): the covariance matrix is assembled, factorised and solved on the
 device through the C ABI (include/stheno_b200.h) and never exists on the host.
@@ -131,7 +131,7 @@ class FiniteGP:
     def factor(self) -> _Factor:
         if self.post is not None:
             if not isinstance(self.post, PosteriorGP):
-                raise NotImplementedError("joint sampling from an approximate (VFE) posterior is not on the B200 path yet")
+                raise NotImplementedError("joint sampling from an approximate (VFE) posterior is not on the CUDA path yet")
             if self._factor is None:
                 # cholesky(cov(f_post(x*, noise))): posterior covariance formed and factorised on device
                 post = self.post
@@ -440,7 +440,7 @@ def posterior(fx, y):
         # instead; same distribution).  One joint factorisation on the device.
         p1 = fx.post
         if not isinstance(p1, PosteriorGP):
-            raise NotImplementedError("posterior of an approximate (VFE) posterior is not on the B200 path")
+            raise NotImplementedError("posterior of an approximate (VFE) posterior is not on the CUDA path")
         n1, n2 = npoints(p1.x), len(fx)
         joint = FiniteGP(p1.prior, _stack_inputs(p1.prior, p1.x, fx.x), _stack_noise(n1, p1.noise, n2, fx.noise))
         return PosteriorGP(joint, np.concatenate([p1.y, np.asarray(y, dtype=np.float64)]))

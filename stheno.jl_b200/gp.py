@@ -1,7 +1,7 @@
-"""GP nodes, affine transformations and *plan lowering* for the B200 hot path.
+"""GP nodes, affine transformations and *plan lowering* for the CUDA hot path.
 
 Host-side mirror of the reference's node types and operator surface
-(/root/reference/src/gp/{util,atomic_gp,derived_gp}.jl, src/affine_transformations/*.jl,
+(Stheno.jl src/gp/{util,atomic_gp,derived_gp}.jl, src/affine_transformations/*.jl,
 src/gaussian_process_probabilistic_programme.jl) -- same names, argument meaning and errors --
 but NOT its evaluation strategy.  The reference evaluates `cov(f_p, f_q, x, x')` by an id-ordered
 recursion that materialises an N x N' matrix per node (src/gp/derived_gp.jl:31-59).  Here every
@@ -42,7 +42,7 @@ class Kernel:
 
     def __mul__(self, c):
         if isinstance(c, Kernel):
-            raise NotImplementedError("kernel products are outside the B200 hot-path scope")
+            raise NotImplementedError("kernel products are outside the CUDA hot-path scope")
         return ScaledKernel(self, float(c))
 
     def lowered(self):
@@ -465,7 +465,7 @@ def _as_point_major(z, scale: float):
     else:
         a = np.asarray(z)
         if a.dtype == np.float32:
-            raise NotImplementedError("Float32 inputs: SB_F32 path is reserved, not built in round 1")
+            raise NotImplementedError("Float32 inputs: SB_F32 path is reserved, not built")
         a = np.ascontiguousarray(a, dtype=np.float64).reshape(-1, 1)
     if scale != 1.0:
         a = a * scale

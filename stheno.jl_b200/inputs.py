@@ -1,6 +1,6 @@
 """Input containers of the hot path: GPPPInput, BlockData, ColVecs, split.
 
-Host-side mirror of /root/reference/src/input_collection_types.jl:24-95 and
+Host-side mirror of Stheno.jl src/input_collection_types.jl:24-95 and
 src/gaussian_process_probabilistic_programme.jl:121-135.  Integer/index semantics are
 bit-exact requirements (tests/test_inputs.py ports test/input_collection_types.jl:4-49).
 Indices are 0-based here (Python); `eachindex` / `block_ranges` return the reference's 1-based

@@ -465,7 +465,7 @@ function timings(; reset::Bool=false)
     t[]
 end
 
-# "trailing" => 0 (fp64 DMMA) | 1 (tcgen05 int8 Ozaki slices)
+# "trailing" => 0 (fp64 DMMA) | 1 (int8 Ozaki slices on wgmma); default 0
 set_option!(key::AbstractString, value::Integer) =
     check(ccall((:sb_ctx_set_option, LIB), Int32, (Ptr{Cvoid}, Cstring, Int64), ctx().h, key, value))
 

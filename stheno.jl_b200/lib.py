@@ -1,6 +1,6 @@
 """ctypes binding of libstheno_b200.so -- the same symbols the Julia shim `ccall`s
-(julia/SthenoB200.jl).  There is NO fallback: if the library is missing or the device is not a
-B200 the product path raises."""
+(julia/SthenoB200.jl).  There is NO fallback: if the library is missing or the device is not an
+H100 (sm_90) the product path raises."""
 from __future__ import annotations
 
 import ctypes as C
@@ -181,7 +181,7 @@ class Context:
         return t.asdict()
 
     def set_option(self, key: str, value: int):
-        """"trailing": 0 = fp64 DMMA, 1 = tcgen05 int8 Ozaki trailing update; "fine_timing": 0/1."""
+        """"trailing": 0 = fp64 DMMA, 1 = int8 Ozaki (wgmma) trailing update; "fine_timing": 0/1."""
         check(load().sb_ctx_set_option(self.h, key.encode(), int(value)))
 
     def mark(self, slot):

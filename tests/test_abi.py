@@ -25,7 +25,7 @@ def test_library_exports_every_declared_symbol():
 
 
 def test_no_gpu_fails_loudly():
-    """Without a B200 the product path must raise, never fall back to a CPU implementation."""
+    """Without a GPU the product path must raise, never fall back to a CPU implementation."""
     import numpy as np
     import pytest
     import torch

@@ -1,8 +1,9 @@
 """CPU pins for the numerical schemes the CUDA library uses in place of LAPACK's dpotrf / dtrsm (the reference's
 `cholesky(Symmetric(cov(fx)))`, SURVEY.md App. A): the int8 digit-plane product, the wide panel phase and the
 peer-to-peer exchange protocol -- restated in NumPy in oracle/device_algorithms.py and checked here against
-exact integer arithmetic, LAPACK and randomised interleavings.  The device kernels are compared with the same
-quantities on the GPU (tools/oz_test.cu: exact digit products; tests/test_gpu_parity.py: the oracle)."""
+exact integer arithmetic, LAPACK and randomised interleavings.  The device kernels are compared with the
+oracle and with LAPACK on the GPU (tests/test_gpu_parity.py), which checks their end results, not the raw
+int32 digit products."""
 from fractions import Fraction
 
 import numpy as np

@@ -11,7 +11,7 @@ from models import f3_model, mixing_model, rich_model, toy_model
 
 pytestmark = pytest.mark.gpu
 RTOL = 1e-10
-DEFAULT_TRAILING = 1   # library default: tcgen05 int8 Ozaki trailing update (0 = fp64 DMMA)
+DEFAULT_TRAILING = 0   # library default: fp64 DMMA trailing update (1 = int8 Ozaki on wgmma)
 
 
 def both(sb, orc, builder):
@@ -207,7 +207,7 @@ def test_vfe_large_m_config4_shape(sb, orc, n, m, trailing):
     """Config-4 geometry (pseudo-points on a unit grid in the observed process, jitter 1e-9 on K_uu,
     x ~ U(0, M), sigma^2 = 0.1) at M = 1024 / 4096: multi-block M x M factors (8 / 32 blocks), several
     16384-row observation chunks; elbo, dtc and the approximate posterior against the oracle, on both
-    the DMMA and the tcgen05 paths."""
+    the DMMA and the int8 Ozaki paths."""
     rng = np.random.default_rng(n + m)
     x = rng.uniform(0, m, n)
     z = np.arange(m) + 0.5
@@ -334,9 +334,9 @@ def test_config2_full_size_properties(sb):
     assert -1e6 < lp < 0
 
 
-def test_config2_full_size_tcgen05_vs_dmma(sb):
+def test_config2_full_size_ozaki_vs_dmma(sb):
     """BASELINE config 2 at full size (N = 65536): the two independent implementations of the O(N^3)
-    -- fp64 DMMA and tcgen05 int8 Ozaki slices -- must agree on logpdf and on the posterior mean /
+    -- fp64 DMMA and int8 Ozaki slices on wgmma -- must agree on logpdf and on the posterior mean /
     variance at 4096 test points to the north-star tolerance (rtol 1e-10)."""
     import bench
     n, ns = 65536, 4096
@@ -516,7 +516,7 @@ def test_vfe_approx_posterior_cov(sb, orc):
 
 @pytest.fixture
 def ozaki_ctx(sb):
-    """Route the trailing updates of the default context through the tcgen05 int8-Ozaki kernel."""
+    """Route the trailing updates of the default context through the int8 Ozaki (wgmma) kernel."""
     ctx = sb.default_context()
     ctx.set_option("trailing", 1)
     try:
@@ -526,8 +526,8 @@ def ozaki_ctx(sb):
 
 
 @pytest.mark.parametrize("n", [2500, 4096])
-def test_tcgen05_ozaki_trailing_update_parity(sb, orc, ozaki_ctx, n):
-    """fp64 Cholesky whose trailing SYRK runs as 28 int8 tcgen05 MMAs per fp64 MMA (ozaki.cu):
+def test_int8_ozaki_trailing_update_parity(sb, orc, ozaki_ctx, n):
+    """fp64 Cholesky whose trailing SYRK runs as 28 int8 wgmma MMAs per fp64 MMA (ozaki.cu):
     the factor must agree with LAPACK to 1e-12 and logpdf / posterior with the oracle to 1e-10."""
     import scipy.linalg as sla
     rng = np.random.default_rng(41)
@@ -538,7 +538,7 @@ def test_tcgen05_ozaki_trailing_update_parity(sb, orc, ozaki_ctx, n):
     t0 = ozaki_ctx.timings(reset=True)
     lp, lpo = sb.logpdf(fxs, y), orc.logpdf(fxo, y)
     tm = ozaki_ctx.timings()
-    assert tm["trailing_int8_ops"] > 0, "the tcgen05 path did not run"
+    assert tm["trailing_int8_ops"] > 0, "the int8 Ozaki path did not run"
     assert abs(lp - lpo) <= RTOL * abs(lpo), (lp, lpo)
     L = fxs.factor().to_dense_L()
     Lref = sla.cholesky(orc.cov(fxo), lower=True)
@@ -550,7 +550,7 @@ def test_tcgen05_ozaki_trailing_update_parity(sb, orc, ozaki_ctx, n):
 
 
 def test_dmma_trailing_update_parity(sb, orc):
-    """The fp64 DMMA path (SB_TRAILING=dmma / option trailing=0) stays covered now that tcgen05 is the default."""
+    """The fp64 DMMA path (SB_TRAILING=dmma / option trailing=0, the default) against LAPACK and the oracle."""
     import scipy.linalg as sla
     rng = np.random.default_rng(43)
     n = 3000
@@ -574,7 +574,7 @@ def test_dmma_trailing_update_parity(sb, orc):
         ctx.set_option("trailing", DEFAULT_TRAILING)
 
 
-def test_tcgen05_ozaki_gppp_badly_scaled_rows(sb, orc, ozaki_ctx):
+def test_int8_ozaki_gppp_badly_scaled_rows(sb, orc, ozaki_ctx):
     """Rows of very different magnitude (function-scaled processes, heteroscedastic noise): the per-row
     power-of-two scaling of the digit planes must keep fp64-level accuracy."""
     rng = np.random.default_rng(42)

@@ -1,5 +1,5 @@
 """BlockData / GPPPInput / split: bit-exact integer semantics.
-Ports /root/reference/test/input_collection_types.jl:4-49 and
+Ports Stheno.jl test/input_collection_types.jl:4-49 and
 test/gaussian_process_probabilistic_programme.jl:3-15 (+ the split doctest, gppp.jl:90-102),
 for BOTH the product's host classes and the oracle's."""
 import numpy as np

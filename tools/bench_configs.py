@@ -5,7 +5,7 @@
   config 4 (2 GPUs):  elbo with M = 4096 pseudo-points, N = 131072 SE kernel: K_uu / K_uf + low-rank Cholesky,
                       approximate-posterior mean / var at 4096 points.  torchrun --nproc-per-node 2 ... --config 4
 
-Parity: config 3 -- residual identity (K + s2 I) alpha = delta on a subset + dmma-vs-tcgen05 agreement;
+Parity: config 3 -- residual identity (K + s2 I) alpha = delta on a subset + dmma-vs-ozaki agreement;
 config 4 -- the CPU oracle's elbo / dtc at full size (Kuf is 4.3 GB on the host: ~1 min with 64 threads) when
 --oracle is given, else cross-check between the two device paths.  One JSON line per config on stdout.
 """
@@ -66,7 +66,7 @@ def config3(args):
     obs = sb.BlockData(*[sb.GPPPInput(nm, v) for nm, v in zip(names, xs)])
     tst = sb.BlockData(*[sb.GPPPInput(nm, v) for nm, v in zip(names, xt)])
     res = {}
-    for mode, name in ((1, "tcgen05"), (0, "dmma")):
+    for mode, name in ((1, "ozaki"), (0, "dmma")):
         ctx.set_option("trailing", mode)
 
         def step():
@@ -79,7 +79,7 @@ def config3(args):
         (lp, m, v, post), t = timed(step, 2, torch.cuda.synchronize)
         tm = ctx.timings()
         res[name] = dict(lp=lp, m=m, v=v, t=t, tm=tm, post=post)
-    a, b = res["tcgen05"], res["dmma"]
+    a, b = res["ozaki"], res["dmma"]
     # residual identity on a subset of the training points (zero-mean prior)
     sel = [np.arange(0, nb, 97) for _ in range(3)]
     idx = np.concatenate([s + nb * k for k, s in enumerate(sel)])
@@ -87,13 +87,13 @@ def config3(args):
     alpha = a["post"].alpha
     resid = float(np.max(np.abs(sb.mean(a["post"], sub) - (y[idx] - 0.1 * alpha[idx]))))
     n = 3 * nb
-    out = {"config": 3, "workload": f"GPPP f3=f1+f2 (SE + Matern52) over BlockData, 3x{nb} inputs (N={n}) fp64, 1xB200: "
+    out = {"config": 3, "workload": f"GPPP f3=f1+f2 (SE + Matern52) over BlockData, 3x{nb} inputs (N={n}) fp64, 1 GPU: "
                                     "block cross-cov assembly + joint Cholesky + logpdf + posterior at 3x1024 points",
-           "points_per_s_tcgen05": n / a["t"], "s_per_step_tcgen05": a["t"], "points_per_s_dmma": n / b["t"], "s_per_step_dmma": b["t"],
-           "logpdf_tcgen05": a["lp"], "logpdf_dmma": b["lp"], "logpdf_rel_diff": abs(a["lp"] - b["lp"]) / abs(b["lp"]),
+           "points_per_s_ozaki": n / a["t"], "s_per_step_ozaki": a["t"], "points_per_s_dmma": n / b["t"], "s_per_step_dmma": b["t"],
+           "logpdf_ozaki": a["lp"], "logpdf_dmma": b["lp"], "logpdf_rel_diff": abs(a["lp"] - b["lp"]) / abs(b["lp"]),
            "mean_max_abs_diff": float(np.max(np.abs(a["m"] - b["m"]))), "var_max_rel_diff": float(np.max(np.abs(a["v"] - b["v"]) / np.abs(b["v"]))),
            "residual_identity_max_abs": resid,
-           "phases_ms_tcgen05": {k: a["tm"][k] / 3 for k in ("assemble_ms", "trailing_ms", "solve_ms", "predict_ms")},
+           "phases_ms_ozaki": {k: a["tm"][k] / 3 for k in ("assemble_ms", "trailing_ms", "solve_ms", "predict_ms")},
            "n_gpus": world}
     if rank == 0:
         print(json.dumps(out))
@@ -116,7 +116,7 @@ def config4(args):
         if dist is not None:
             dist.barrier()
     res = {}
-    for mode, name in ((1, "tcgen05"), (0, "dmma")):
+    for mode, name in ((1, "ozaki"), (0, "dmma")):
         ctx.set_option("trailing", mode)
 
         def step():
@@ -126,11 +126,11 @@ def config4(args):
             return ap.elbo, ap.dtc, mm, vv
         (e, d, mm, vv), t = timed(step, 2, sync)
         res[name] = dict(elbo=e, dtc=d, m=mm, v=vv, t=t)
-    a, b = res["tcgen05"], res["dmma"]
+    a, b = res["ozaki"], res["dmma"]
     out = {"config": 4, "workload": f"elbo(VFE) with M={m} pseudo-points on a unit grid (jitter 1e-9), N={n} SE kernel fp64, "
-                                    f"{world}xB200: K_uu / K_uf + two MxM Choleskys + approximate-posterior mean/var at 4096 points",
-           "points_per_s_tcgen05": n / a["t"], "s_per_step_tcgen05": a["t"], "points_per_s_dmma": n / b["t"], "s_per_step_dmma": b["t"],
-           "elbo_tcgen05": a["elbo"], "elbo_dmma": b["elbo"], "dtc_tcgen05": a["dtc"],
+                                    f"{world} GPU(s): K_uu / K_uf + two MxM Choleskys + approximate-posterior mean/var at 4096 points",
+           "points_per_s_ozaki": n / a["t"], "s_per_step_ozaki": a["t"], "points_per_s_dmma": n / b["t"], "s_per_step_dmma": b["t"],
+           "elbo_ozaki": a["elbo"], "elbo_dmma": b["elbo"], "dtc_ozaki": a["dtc"],
            "elbo_rel_diff_paths": abs(a["elbo"] - b["elbo"]) / abs(b["elbo"]),
            "mean_max_abs_diff_paths": float(np.max(np.abs(a["m"] - b["m"]))), "n_gpus": world}
     if args.oracle and rank == 0:

@@ -1,6 +1,6 @@
 // Microbenchmark of the DMMA inner loop fed from shared memory (no global traffic): isolates
 // whether the LDS.64 fragment loads + DMMA.8x8x4 issue pattern of gemm_nt.cu can reach the
-// measured 37.1 TFLOP/s DMMA peak.  Variants: warp tile shape, CTAs/SM, fragment reuse.
+// DMMA peak that tools/mb_fp64_peak measures.  Variants: warp tile shape, CTAs/SM, fragment reuse.
 #include <cstdio>
 #include <cstdlib>
 #include <cuda_runtime.h>

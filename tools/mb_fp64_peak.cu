@@ -1,6 +1,6 @@
-// Microbenchmark: fp64 peak on B200 (sm_100a) for DFMA and the mma.sync f64 shapes.
-// Builder-measured denominator for the Cholesky trailing-update roofline
-// (MEASURED_PEAKS.json has only bf16 + HBM).  Usage: ./mb_fp64_peak [iters]
+// Microbenchmark: fp64 peak (sm_90a) for DFMA and the mma.sync f64 shapes.
+// Measured denominator for the Cholesky trailing-update roofline.
+// Usage: ./mb_fp64_peak [iters]
 #include <cstdio>
 #include <cstdlib>
 #include <cuda_runtime.h>

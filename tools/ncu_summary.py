@@ -1,4 +1,4 @@
-"""Summarise one kernel of an .ncu-rep (read here, on the CPU box): python tools/ncu_summary.py report.ncu-rep [title]"""
+"""Summarise one kernel of an .ncu-rep (needs only the ncu CLI, no GPU): python tools/ncu_summary.py report.ncu-rep [title]"""
 import csv, subprocess, sys
 
 rep = sys.argv[1]
