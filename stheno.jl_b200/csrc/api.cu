@@ -29,10 +29,6 @@ int32_t cuda_fail(cudaError_t e, const char* what, const char* file, int line) {
 
 using namespace sb;
 
-#ifndef SB_DEFAULT_TRAILING
-#define SB_DEFAULT_TRAILING 0   /* fp64 DMMA trailing update, the faster path on H100 (SB_TRAILING=ozaki selects int8 Ozaki) */
-#endif
-
 // NCCL is bound lazily with dlopen (only when world > 1): a single-GPU / Julia user never loads
 // it, and inside a Python process that also imports torch the already-loaded libnccl.so.2
 // (torch bundles its own) is reused instead of clashing with the system copy.
@@ -92,10 +88,9 @@ struct sb_ctx {
     cudaStream_t xstream[4] = {nullptr, nullptr, nullptr, nullptr};  // column-exchange streams, one per owner in flight
     sb_timings tm{};
     bool fine_timing = true;
-    int trailing_mode = 0;   // 0: fp64 DMMA (mma.sync), 1: int8 Ozaki slices on wgmma (ozaki.cu)
+    // 0: fp64 DMMA (mma.sync), the faster path on H100 and the default; 1: int8 Ozaki slices on wgmma (ozaki.cu)
+    int trailing_mode = 0;
     int num_sms = 132;
-    int sweep_variant = 2;      // persistent sweep variant (solve.cu): 2 = diag CTA + L2 prefetch
-    bool legacy_solve = false;  // SB_SOLVE=legacy: two launches per block instead of the persistent sweep
     cudaEvent_t marks[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
     // peer-to-peer panel exchange over NVLink (multi-GPU, see "P2P panel exchange" below)
     struct P2PState {
@@ -168,7 +163,8 @@ struct sb_factor {
     bool has_alpha = false;
     double logdet = 0.0;
     size_t bytes_L = 0, bytes_invL = 0, bytes_ld = 0, bytes_panel = 0, bytes_alpha = 0, bytes_ldiag = 0;
-    // int8 Ozaki trailing update (ozaki.cu): two sets (look-ahead) of int8 digit planes + row scales
+    // int8 Ozaki trailing update (ozaki.cu): two sets (look-ahead) of int8 digit planes + row scales, and the
+    // wide panel phase's buffers below; all allocated together
     bool oz = false;
     signed char* oz_planes[2] = {nullptr, nullptr};
     double* oz_scale[2] = {nullptr, nullptr};
@@ -181,9 +177,8 @@ struct sb_factor {
     bool vcache_valid = false;
     OzMaps oz_maps[2];
     size_t bytes_oz_planes = 0;
-    // wide panel phase (int8 Ozaki path, see wide_panel_phase): dense scratch of the step's 512 x 512 diagonal block
-    // stacked over an identity (input and result copies), inv(L_512) and its digit planes
-    bool wide = false;
+    // wide panel phase (see wide_diag_phase): dense scratch of the step's 512 x 512 diagonal block stacked over an
+    // identity (input and result copies), inv(L_512) and its digit planes
     double* wide_D = nullptr;        // [2][1024 x 512], ld 1024
     double* wide_W = nullptr;        // 512 x 512, column-major
     signed char* wide_wp = nullptr;  // digit planes of wide_W  [7][512][512]
@@ -598,43 +593,34 @@ static int32_t bcast_panel(sb_ctx* c, sb_factor* f, int64_t k, double* Pslab, si
     return SB_OK;
 }
 
-// Multi-GPU factorisation with look-ahead.  Stream 1 (c->stream) runs the trailing updates,
-// stream 2 (c->stream2) the panel phases (column catch-up, potrf, TRSM, NCCL broadcast, untile).
+// Multi-GPU DMMA factorisation with look-ahead.  Stream 1 (c->stream) runs the trailing updates,
+// stream 2 (c->stream2) the panel phases (column catch-up, potrf, TRSM, panel exchange, untile).
 // The trailing update of outer step s is split into T^A (the 4 block columns that form the NEXT
 // step's panels; full grid) and T^B (everything to the right; persistent grid minus
 // LOOKAHEAD_SMS SMs).  Panel phase s+1 starts as soon as T^A_s is done and overlaps T^B_s, so the
 // serial potrf/TRSM/broadcast chain leaves the critical path.  Two sets of tiled panel buffers.
 constexpr int LOOKAHEAD_SMS = 8;
-constexpr int OZ_CHUNK_TILES = 8;   // tiles per CTA of a chunked T^B launch (multi-GPU default)
 
 // How many SMs T^B leaves to the concurrent panel phase.  With a fixed 8 SMs the panel-phase GEMMs
 // (catch-up SYRK, TRSM-as-GEMM: up to ~2000 DMMA half-tiles per outer step) crawl on 16 CTA slots and
 // the panel chain, not the trailing update, can set the pace of the second half of the factorisation.
 // Pick the reservation that balances  T^B * S/(S-r)  against  serial chain + panel GEMM work / r.
-// Per-tile costs: time per SM of one 128 x 64 half-tile with K = 512 (2*128*64*512 flop) at the
-// trailing-update rates bench.py measured at N = 65536 on one H100 80GB (700 W): DMMA 28.1 TFLOP/s,
-// int8 Ozaki 23.0 TFLOP/s fp64-equivalent, over 132 SMs.  The serial-chain and wide-phase latencies
-// below have not been measured on H100.
-constexpr double DMMA_HALF_TILE_US = 39.5, OZ_HALF_TILE_US = 48.1;
-static int pick_lookahead_sms(int num_sms, double tilesB_half, bool oz, int nq_next, int64_t rows_next, int world,
-                              bool wide = false) {
-    const double t_tile_us = oz ? OZ_HALF_TILE_US : DMMA_HALF_TILE_US;   // per half-tile per SM
-    const double serial_us = nq_next * (world > 1 ? 230.0 : 150.0); // potrf + (broadcast latency); unmeasured
+// Per-tile cost: time per SM of one 128 x 64 half-tile with K = 512 (2*128*64*512 flop) at the DMMA
+// trailing-update rate bench.py measured at N = 65536 on one H100 80GB (700 W), 28.1 TFLOP/s over 132 SMs.
+// The serial-chain latencies below have not been measured on H100.
+constexpr double DMMA_HALF_TILE_US = 39.5;
+static int pick_lookahead_sms(int num_sms, double tilesB_half, int nq_next, int64_t rows_next) {
+    const double serial_us = nq_next * 230.0;   // potrf + exchange latency; unmeasured
     // DMMA half-tiles of the next panel phase: TRSM (nq panels) + catch-up (0 + 1 + 2 + 3 segments)
     const double gemm_tiles = (double)nq_next * (rows_next / 64.0) * (1.0 + 0.5 * (nq_next - 1) * 0.5);
-    static const int forced = getenv("SB_LOOKAHEAD_SMS") ? atoi(getenv("SB_LOOKAHEAD_SMS")) : 0;
-    if (forced > 0) return forced < num_sms / 2 ? forced : num_sms / 2;
     const int cand[] = {8, 12, 16, 24, 32, 48, 64};
     int best = LOOKAHEAD_SMS;
     double best_t = 1e30;
     for (int r : cand) {
         if (r >= num_sms / 2) break;
-        const double tB = tilesB_half * t_tile_us / (num_sms - r);
-        // wide phase: potrfs / small products per step (~0.9 ms assumed), then ONE int8 Ozaki product of
-        // (rows / 128) x 8 half-tiles (K = 512) confined to the r free SMs
+        const double tB = tilesB_half * DMMA_HALF_TILE_US / (num_sms - r);
         // (panel-phase GEMM tiles have K = 128: a quarter of a half-tile's work)
-        const double tP = wide ? 900.0 + (world > 1 ? 350.0 : 0.0) + (double)(rows_next / NB) * 8.0 * OZ_HALF_TILE_US / r
-                               : serial_us + gemm_tiles * (DMMA_HALF_TILE_US / 4.0) / r;
+        const double tP = serial_us + gemm_tiles * (DMMA_HALF_TILE_US / 4.0) / r;
         const double t = tB > tP ? tB : tP;
         if (t < best_t - 1e-9) { best_t = t; best = r; }
     }
@@ -643,11 +629,13 @@ static int pick_lookahead_sms(int num_sms, double tilesB_half, bool oz, int nq_n
 
 struct CommEv { cudaEvent_t a, b; };
 
-static int32_t panel_phase(sb_ctx* c, sb_factor* f, int64_t k0, int nq, double* const* Pw, const double* const* Pt,
+// Panels q0 .. q1-1 of the outer step at block column k0: column catch-up, potrf, TRSM, exchange, untile.
+// comm_ev (fine timing): one interval per panel around its exchange (empty on one rank).
+static int32_t panel_phase(sb_ctx* c, sb_factor* f, int64_t k0, int q0, int q1, double* const* Pw, const double* const* Pt,
                            int rank, int world, cudaStream_t st, std::vector<CommEv>* comm_ev, P2PRun* R = nullptr) {
     const bool p2p = R && R->on;
     const int64_t Np = f->Np;
-    for (int q = 0; q < nq; q++) {
+    for (int q = q0; q < q1; q++) {
         const int64_t kq = k0 + q;
         const int64_t mq = Np - (kq + 1) * NB;
         const int owner = (int)(kq % world);
@@ -659,12 +647,12 @@ static int32_t panel_phase(sb_ctx* c, sb_factor* f, int64_t k0, int nq, double* 
             if (mq > 0)
                 launch_trsm_tiled(f->L.blk(kq + 1, kq), f->L.ld(kq), f->invL + kq * (int64_t)NB * NB, Pq, mq, st);
         }
+        CommEv ce{nullptr, nullptr};
+        if (comm_ev && c->fine_timing) {
+            ce.a = c->next_event(); ce.b = c->next_event();
+            SB_CUDA(cudaEventRecord(ce.a, st));
+        }
         if (world > 1) {
-            CommEv ce{nullptr, nullptr};
-            if (comm_ev && c->fine_timing) {
-                ce.a = c->next_event(); ce.b = c->next_event();
-                SB_CUDA(cudaEventRecord(ce.a, st));
-            }
             const size_t slab = mq > 0 ? (size_t)tiled_panel_elems(mq) : 0;
             if (!p2p) {
                 SB_TRY(bcast_panel(c, f, kq, Pq, slab, owner, st));
@@ -674,8 +662,8 @@ static int32_t panel_phase(sb_ctx* c, sb_factor* f, int64_t k0, int nq, double* 
                 SB_TRY(p2p_slot_guard(c, *R, kq, st));
                 SB_TRY(p2p_pull(c, f, *R, kq, owner, tiled_panel_elems((int64_t)q * NB), slab, st));
             }
-            if (ce.a) { SB_CUDA(cudaEventRecord(ce.b, st)); comm_ev->push_back(ce); }
         }
+        if (ce.a) { SB_CUDA(cudaEventRecord(ce.b, st)); comm_ev->push_back(ce); }
         if (mq > 0) launch_untile_panel(Pt[q], q, mq / NB, f->L.blk(kq + 1, kq), f->L.ld(kq), st);
     }
     return SB_OK;
@@ -755,24 +743,19 @@ static int32_t wide_diag_phase(sb_ctx* c, sb_factor* f, int64_t k0, int nq, int 
         }
         // The columns of a step come from different owners: their pulls run side by side, one stream per owner
         // (two columns of the same owner stay in order on one stream, which keeps its counters monotone).
-        static const bool serial = getenv("SB_P2P_SERIAL") != nullptr;
-        if (serial) {
-            for (int q = 0; q < nq; q++) SB_TRY(p2p_exchange_col(c, f, *R, k0 + q, st));
-        } else {
-            cudaEvent_t e0 = c->next_event();
-            SB_CUDA(cudaEventRecord(e0, st));
-            bool used[4] = {false, false, false, false};
-            for (int q = 0; q < nq; q++) {
-                const int xi = (int)((k0 + q) % world) % 4;
-                if (!used[xi]) { SB_CUDA(cudaStreamWaitEvent(c->xstream[xi], e0, 0)); used[xi] = true; }
-                SB_TRY(p2p_exchange_col(c, f, *R, k0 + q, c->xstream[xi]));
-            }
-            for (int xi = 0; xi < 4; xi++) {
-                if (!used[xi]) continue;
-                cudaEvent_t e1 = c->next_event();
-                SB_CUDA(cudaEventRecord(e1, c->xstream[xi]));
-                SB_CUDA(cudaStreamWaitEvent(st, e1, 0));
-            }
+        cudaEvent_t e0 = c->next_event();
+        SB_CUDA(cudaEventRecord(e0, st));
+        bool used[4] = {false, false, false, false};
+        for (int q = 0; q < nq; q++) {
+            const int xi = (int)((k0 + q) % world) % 4;
+            if (!used[xi]) { SB_CUDA(cudaStreamWaitEvent(c->xstream[xi], e0, 0)); used[xi] = true; }
+            SB_TRY(p2p_exchange_col(c, f, *R, k0 + q, c->xstream[xi]));
+        }
+        for (int xi = 0; xi < 4; xi++) {
+            if (!used[xi]) continue;
+            cudaEvent_t e1 = c->next_event();
+            SB_CUDA(cudaEventRecord(e1, c->xstream[xi]));
+            SB_CUDA(cudaStreamWaitEvent(st, e1, 0));
         }
         if (ce.a) { SB_CUDA(cudaEventRecord(ce.b, st)); comm_ev->push_back(ce); }
     }
@@ -834,6 +817,57 @@ static int32_t wide_bulk_phase(sb_ctx* c, sb_factor* f, int64_t k0, int nq, int 
     return SB_OK;
 }
 
+// Start of a factorisation over the IPC-mapped arena: ordinal of every panel among its owner's panels, and (on
+// stream st) a wait until every panel this rank published in earlier factorisations has been pulled by everyone.
+static int32_t p2p_run_begin(sb_ctx* c, sb_factor* f, P2PRun& R, int world, int rank, cudaStream_t st) {
+    const int64_t nblk = f->L.nblk();
+    R.on = true;
+    R.slot_elems = tiled_panel_elems(f->Np);
+    for (int r = 0; r < 8; r++) R.peers.base[r] = c->p2p.peer[r];
+    R.ord.resize(nblk);
+    R.guarded = c->p2p.pub[rank];
+    for (int64_t k = 0; k < nblk; k++) R.ord[k] = ++c->p2p.pub[k % world];
+    p2p_wait_kernel<<<1, 32, 0, st>>>(R.ctr(c), P2P_ACK, world, rank, R.guarded, R.ctr(c) + P2P_ERR);
+    SB_CUDA(cudaGetLastError());
+    return SB_OK;
+}
+
+// End of a two-stream factorisation: the trailing stream waits for the panel stream and the host for both, a
+// timed-out peer exchange fails the factorisation, and the exchange intervals and panel-stream phases (fine
+// timing) are added to comm_ms and panel_chain_ms.
+static int32_t finish_two_streams(sb_ctx* c, const P2PRun& R, const std::vector<CommEv>& comm_ev,
+                                  const std::vector<CommEv>& chain_ev) {
+    cudaEvent_t e_pend = c->next_event();
+    SB_CUDA(cudaEventRecord(e_pend, c->stream2));
+    SB_CUDA(cudaStreamWaitEvent(c->stream, e_pend, 0));
+    SB_CUDA(cudaGetLastError());
+    SB_CUDA(cudaStreamSynchronize(c->stream));
+    if (R.on) {
+        uint32_t err = 0;
+        SB_CUDA(cudaMemcpy(&err, R.ctr(c) + P2P_ERR, sizeof(err), cudaMemcpyDeviceToHost));
+        if (err) {
+            sb::set_error("peer-to-peer panel exchange timed out (a peer rank stopped making progress)");
+            return SB_ERR_NCCL;
+        }
+    }
+    if (c->fine_timing) {
+        // exchange time includes waiting for the owner's panel work on the other ranks
+        for (auto& ce : comm_ev) {
+            float ms = 0;
+            cudaEventElapsedTime(&ms, ce.a, ce.b);
+            c->tm.comm_ms += ms;
+        }
+        for (auto& ce : chain_ev) {
+            float ms = 0;
+            cudaEventElapsedTime(&ms, ce.a, ce.b);
+            c->tm.panel_chain_ms += ms;
+        }
+    }
+    return SB_OK;
+}
+
+// Look-ahead factorisation (see above).  Panels move by the P2P exchange when the arena is mapped, else by the
+// NCCL broadcast.
 static int32_t cholesky_lookahead(sb_ctx* c, sb_factor* f, int world, int rank) {
     const int64_t nblk = f->L.nblk(), Np = f->Np;
     std::vector<CommEv> comm_ev, chain_ev;
@@ -844,35 +878,23 @@ static int32_t cholesky_lookahead(sb_ctx* c, sb_factor* f, int world, int rank) 
     for (int set = 0; set < 2; set++)
         for (int q = 0; q < OUTER_BLOCKS; q++)
             Pt[set][q] = Pw[set][q] = f->panel + (int64_t)(set * OUTER_BLOCKS + q) * tiled_panel_elems(Np);
-    P2PRun R;
-    if (world > 1 && c->p2p.state == 1) {   // panels move by peer copies through the IPC-mapped arena
-        R.on = true;
-        R.slot_elems = tiled_panel_elems(Np);
-        for (int r = 0; r < 8; r++) R.peers.base[r] = c->p2p.peer[r];
-        R.ord.resize(nblk);
-        R.guarded = c->p2p.pub[rank];
-        for (int64_t k = 0; k < nblk; k++) R.ord[k] = ++c->p2p.pub[k % world];
-        for (int set = 0; set < 2; set++)   // the arena slots ARE the tiled panel buffers
-            for (int q = 0; q < OUTER_BLOCKS; q++) Pt[set][q] = Pw[set][q] = R.slot(c->p2p.arena, set * OUTER_BLOCKS + q);
-    }
     std::vector<cudaEvent_t> ev_p(nsteps), ev_a(nsteps), ev_t0(nsteps), ev_t1(nsteps);
     for (int64_t s = 0; s < nsteps; s++) {
         ev_p[s] = c->next_event(); ev_a[s] = c->next_event(); ev_t0[s] = c->next_event(); ev_t1[s] = c->next_event();
     }
-    cudaEvent_t e_start = c->next_event(), e_pend = c->next_event();
+    cudaEvent_t e_start = c->next_event();
     // stream 2 starts after everything already queued on stream 1 (assembly)
     SB_CUDA(cudaEventRecord(e_start, s1));
     SB_CUDA(cudaStreamWaitEvent(s2, e_start, 0));
-    if (R.on) {   // every panel this rank published in earlier factorisations has been pulled by everyone
-        p2p_wait_kernel<<<1, 32, 0, s2>>>(R.ctr(c), P2P_ACK, world, rank, R.guarded, R.ctr(c) + P2P_ERR);
-        SB_CUDA(cudaGetLastError());
+    P2PRun R;
+    if (c->p2p.state == 1) {
+        SB_TRY(p2p_run_begin(c, f, R, world, rank, s2));
+        for (int set = 0; set < 2; set++)   // the arena slots ARE the tiled panel buffers
+            for (int q = 0; q < OUTER_BLOCKS; q++) Pt[set][q] = Pw[set][q] = R.slot(c->p2p.arena, set * OUTER_BLOCKS + q);
     }
     {
         const int nq0 = (int)(nblk < OUTER_BLOCKS ? nblk : OUTER_BLOCKS);
-        SB_TRY(panel_phase(c, f, 0, nq0, Pw[0], Pt[0], rank, world, s2, &comm_ev, &R));
-        if (f->oz)
-            launch_oz_slice(oz_src_tiled(Pt[0], nq0), nq0 - 1, nblk - nq0, (int64_t)NB, Np, f->oz_scale[0], f->oz_expo[0],
-                            f->oz_planes[0], s2);
+        SB_TRY(panel_phase(c, f, 0, 0, nq0, Pw[0], Pt[0], rank, world, s2, &comm_ev, &R));
         SB_CUDA(cudaEventRecord(ev_p[0], s2));
     }
     double flops = 0;
@@ -886,61 +908,30 @@ static int32_t cholesky_lookahead(sb_ctx* c, sb_factor* f, int world, int rank) 
         SB_CUDA(cudaEventRecord(ev_t0[s], s1));
         if (jt < nblk) {
             const int64_t jA = jt + OUTER_BLOCKS < nblk ? jt + OUTER_BLOCKS : nblk;
-            auto trailing = [&](int64_t jlo, int64_t jhi, int reserve) -> int32_t {
-                if (f->oz) {
-                    if (launch_syrk_ozaki(f->L, k0, nq, jlo, jhi, rank, world, &f->oz_maps[set], f->oz_scale[set],
-                                          s1, reserve) != 0) {
-                        sb::set_error("int8 Ozaki trailing kernel could not be launched");
-                        return SB_ERR_CUDA;
-                    }
-                } else {
-                    launch_syrk_packed(f->L, k0, Pt[set], nq, jlo, jhi, rank, world, s1, reserve);
-                }
-                return SB_OK;
-            };
-            SB_TRY(trailing(jt, jA, 0));                                                   // T^A: next panels' columns
+            launch_syrk_packed(f->L, k0, Pt[set], nq, jt, jA, rank, world, s1);              // T^A: next panels' columns
             SB_CUDA(cudaEventRecord(ev_a[s], s1));
             if (s + 1 < nsteps) {
                 const int nq1 = (int)(nblk - jt < OUTER_BLOCKS ? nblk - jt : OUTER_BLOCKS);
                 SB_CUDA(cudaStreamWaitEvent(s2, ev_a[s], 0));
                 CommEv ch{nullptr, nullptr};
                 if (c->fine_timing) { ch.a = c->next_event(); ch.b = c->next_event(); SB_CUDA(cudaEventRecord(ch.a, s2)); }
-                SB_TRY(panel_phase(c, f, jt, nq1, Pw[set ^ 1], Pt[set ^ 1], rank, world, s2, &comm_ev, &R));
-                if (f->oz)  // digit planes of the trailing rows of the panels just factored (block rows >= jt + nq1)
-                    launch_oz_slice(oz_src_tiled(Pt[set ^ 1], nq1), nq1 - 1, nblk - (jt + nq1), (jt + 1) * (int64_t)NB, Np,
-                                    f->oz_scale[set ^ 1], f->oz_expo[set ^ 1], f->oz_planes[set ^ 1], s2);
+                SB_TRY(panel_phase(c, f, jt, 0, nq1, Pw[set ^ 1], Pt[set ^ 1], rank, world, s2, &comm_ev, &R));
                 SB_CUDA(cudaEventRecord(ev_p[s + 1], s2));
                 if (ch.a) { SB_CUDA(cudaEventRecord(ch.b, s2)); chain_ev.push_back(ch); }
             }
             if (jA < nblk) {                                                                // T^B
                 const double tilesB = 2.0 * (double)syrk_packed_tiles(nblk, k0, jA, nblk, rank, world);
                 const int nq1 = (int)(nblk - jt < OUTER_BLOCKS ? nblk - jt : OUTER_BLOCKS);
-                // T^B next to a panel phase: either a persistent grid that leaves `reserve` SMs free, or
-                // (int8 Ozaki path, SB_OZ_CHUNK > 0) short-lived CTAs of `chunk` tiles each, which hand SMs to
-                // the high-priority panel stream as they retire.
-                static const int chunk_env = getenv("SB_OZ_CHUNK") ? atoi(getenv("SB_OZ_CHUNK")) : 0;
-                int reserve = (s + 1 < nsteps)
-                    ? pick_lookahead_sms(c->num_sms, tilesB, f->oz, nq1, Np - (jt + 1) * NB, world) : 0;
-                if (reserve > 0 && f->oz && chunk_env > 0) reserve = -chunk_env;
-                SB_TRY(trailing(jA, nblk, reserve));
+                const int reserve = (s + 1 < nsteps)
+                    ? pick_lookahead_sms(c->num_sms, tilesB, nq1, Np - (jt + 1) * NB) : 0;
+                launch_syrk_packed(f->L, k0, Pt[set], nq, jA, nblk, rank, world, s1, reserve);
             }
             int64_t tiles = syrk_packed_tiles(nblk, k0, jt, nblk, rank, world);
             if (tiles > 0) { flops += (double)tiles * 2.0 * NB * NB * ((double)nq * NB); nlaunch++; }
         }
         SB_CUDA(cudaEventRecord(ev_t1[s], s1));
     }
-    SB_CUDA(cudaEventRecord(e_pend, s2));
-    SB_CUDA(cudaStreamWaitEvent(s1, e_pend, 0));
-    SB_CUDA(cudaGetLastError());
-    SB_CUDA(cudaStreamSynchronize(s1));
-    if (R.on) {
-        uint32_t err = 0;
-        SB_CUDA(cudaMemcpy(&err, R.ctr(c) + P2P_ERR, sizeof(err), cudaMemcpyDeviceToHost));
-        if (err) {
-            sb::set_error("peer-to-peer panel exchange timed out (a peer rank stopped making progress)");
-            return SB_ERR_NCCL;
-        }
-    }
+    SB_TRY(finish_two_streams(c, R, comm_ev, chain_ev));
     if (c->fine_timing) {
         for (int64_t s = 0; s < nsteps; s++) {
             float ms = 0;
@@ -951,22 +942,9 @@ static int32_t cholesky_lookahead(sb_ctx* c, sb_factor* f, int world, int rank) 
         float ms = 0;
         cudaEventElapsedTime(&ms, e_start, ev_p[0]);
         c->tm.panel_ms += ms;  // only the first, un-hidden panel phase is on the critical path
-        // NCCL time on the look-ahead stream (overlapped with T^B except for the first phase):
-        // the interval includes waiting for the owner's potrf/TRSM on the other ranks
-        for (auto& ce : comm_ev) {
-            float cm = 0;
-            cudaEventElapsedTime(&cm, ce.a, ce.b);
-            c->tm.comm_ms += cm;
-        }
-        for (auto& ce : chain_ev) {   // total duration of the look-ahead panel phases (stream 2)
-            float cm = 0;
-            cudaEventElapsedTime(&cm, ce.a, ce.b);
-            c->tm.panel_chain_ms += cm;
-        }
     }
     c->tm.trailing_flops += flops;
     c->tm.trailing_launches += nlaunch;
-    if (f->oz) c->tm.trailing_int8_ops += 28.0 * flops;
     return SB_OK;
 }
 
@@ -975,34 +953,21 @@ static int32_t cholesky_lookahead(sb_ctx* c, sb_factor* f, int world, int rank) 
 // and on the panel stream, under T^B_s part 1: column exchange + diagonal block + inv(L_512) of step s+1.
 // Part 1 is sized to the duration of that serial chain, so the SM reservation costs ~ 8 / 132 of the GPU for that long per step.
 static int32_t cholesky_wide(sb_ctx* c, sb_factor* f, int world, int rank) {
-    const int64_t nblk = f->L.nblk(), Np = f->Np;
+    const int64_t nblk = f->L.nblk();
     std::vector<CommEv> comm_ev, chain_ev, bulk_ev;
     cudaStream_t s1 = c->stream, s2 = c->stream2;
     const int64_t nsteps = (nblk + OUTER_BLOCKS - 1) / OUTER_BLOCKS;
-    P2PRun R;
-    if (world > 1) {
-        R.on = true;
-        R.slot_elems = tiled_panel_elems(Np);
-        for (int r = 0; r < 8; r++) R.peers.base[r] = c->p2p.peer[r];
-        R.ord.resize(nblk);
-        R.guarded = c->p2p.pub[rank];
-        for (int64_t k = 0; k < nblk; k++) R.ord[k] = ++c->p2p.pub[k % world];
-    }
     std::vector<cudaEvent_t> ev_d(nsteps), ev_a(nsteps), ev_t0(nsteps), ev_t1(nsteps);
     for (int64_t s = 0; s < nsteps; s++) {
         ev_d[s] = c->next_event(); ev_a[s] = c->next_event(); ev_t0[s] = c->next_event(); ev_t1[s] = c->next_event();
     }
-    cudaEvent_t e_start = c->next_event(), e_pend = c->next_event();
+    cudaEvent_t e_start = c->next_event();
     SB_CUDA(cudaEventRecord(e_start, s1));
     SB_CUDA(cudaStreamWaitEvent(s2, e_start, 0));
-    if (R.on) {   // every column this rank published in earlier factorisations has been pulled by everyone
-        p2p_wait_kernel<<<1, 32, 0, s2>>>(R.ctr(c), P2P_ACK, world, rank, R.guarded, R.ctr(c) + P2P_ERR);
-        SB_CUDA(cudaGetLastError());
-    }
-    static const int r_env = getenv("SB_LOOKAHEAD_SMS") ? atoi(getenv("SB_LOOKAHEAD_SMS")) : 0;
-    static const int p1_env = getenv("SB_WIDE_P1_US") ? atoi(getenv("SB_WIDE_P1_US")) : 0;
-    const int reserve_p1 = r_env > 0 ? r_env : LOOKAHEAD_SMS;
-    const double chain_us = p1_env > 0 ? (double)p1_env : (world > 1 ? 2500.0 : 1200.0);
+    P2PRun R;
+    if (world > 1) SB_TRY(p2p_run_begin(c, f, R, world, rank, s2));
+    const int reserve_p1 = LOOKAHEAD_SMS;
+    const double chain_us = world > 1 ? 2500.0 : 1200.0;
     const int64_t p1_tiles = (int64_t)(chain_us / 14.5 * (c->num_sms - reserve_p1));   // half-tiles T^B part 1 should last
 
     auto bulk = [&](int64_t s) -> int32_t {      // panel solve + digit planes of step s, trailing stream
@@ -1063,18 +1028,7 @@ static int32_t cholesky_wide(sb_ctx* c, sb_factor* f, int world, int rank) {
         }
         SB_CUDA(cudaEventRecord(ev_t1[s], s1));
     }
-    SB_CUDA(cudaEventRecord(e_pend, s2));
-    SB_CUDA(cudaStreamWaitEvent(s1, e_pend, 0));
-    SB_CUDA(cudaGetLastError());
-    SB_CUDA(cudaStreamSynchronize(s1));
-    if (R.on) {
-        uint32_t err = 0;
-        SB_CUDA(cudaMemcpy(&err, R.ctr(c) + P2P_ERR, sizeof(err), cudaMemcpyDeviceToHost));
-        if (err) {
-            sb::set_error("peer-to-peer column exchange timed out (a peer rank stopped making progress)");
-            return SB_ERR_NCCL;
-        }
-    }
+    SB_TRY(finish_two_streams(c, R, comm_ev, chain_ev));
     if (c->fine_timing) {
         double tr = 0, bk = 0;
         for (int64_t s = 0; s < nsteps; s++) {
@@ -1093,16 +1047,6 @@ static int32_t cholesky_wide(sb_ctx* c, sb_factor* f, int world, int rank) {
         float ms = 0;
         cudaEventElapsedTime(&ms, e_start, ev_d[0]);
         c->tm.panel_ms += ms;                  // the first serial phase is not hidden
-        for (auto& ce : comm_ev) {             // column exchange incl. waiting for the owners' T^A
-            float cm = 0;
-            cudaEventElapsedTime(&cm, ce.a, ce.b);
-            c->tm.comm_ms += cm;
-        }
-        for (auto& ce : chain_ev) {
-            float cm = 0;
-            cudaEventElapsedTime(&cm, ce.a, ce.b);
-            c->tm.panel_chain_ms += cm;
-        }
     }
     c->tm.trailing_flops += flops;
     c->tm.trailing_launches += nlaunch;
@@ -1115,15 +1059,14 @@ static int32_t sync_info(sb_ctx* c, sb_factor* f);
 int32_t cholesky_packed(sb_ctx* c, sb_factor* f, bool force_local = false) {
     const int64_t nblk = f->L.nblk();
     const int world = force_local ? 1 : c->world, rank = force_local ? 0 : c->rank;
-    // look-ahead (panel phase of step s+1 on stream 2 under the big trailing update of step s) also
-    // pays on ONE GPU: the serial potrf/TRSM chain leaves the critical path
-    // (with the DMMA trailing kernel on ONE GPU the 8 SMs the look-ahead reserves cost about as much
-    //  as the hidden panel chain saves, so it is used for world > 1 and for the int8 Ozaki trailing kernel)
-    static const bool no_la = getenv("SB_NO_LOOKAHEAD") != nullptr;
-    static const bool force_la = getenv("SB_FORCE_LOOKAHEAD") != nullptr;
-    if (!no_la && nblk > OUTER_BLOCKS && (world > 1 || f->oz || force_la)) {
+    // Overlapping the panel chain with the trailing update (two streams) pays for the int8 Ozaki path, and on
+    // several GPUs, where the chain includes the panel exchange.  With the DMMA trailing kernel on ONE GPU the
+    // 8 SMs the look-ahead reserves cost about as much as the hidden panel chain saves: the serial driver below.
+    // int8 Ozaki (f->oz: nblk > 2 * OUTER_BLOCKS) uses the wide panel phase, which on several GPUs needs the
+    // IPC-mapped arena; without it the DMMA look-ahead factors (P2P exchange or NCCL broadcast).
+    if (world == 1 ? f->oz : nblk > OUTER_BLOCKS) {
         if (world > 1) SB_TRY(p2p_ensure(c, f->Np));
-        if (f->wide && (world == 1 || c->p2p.state == 1)) SB_TRY(cholesky_wide(c, f, world, rank));
+        if (f->oz && (world == 1 || c->p2p.state == 1)) SB_TRY(cholesky_wide(c, f, world, rank));
         else SB_TRY(cholesky_lookahead(c, f, world, rank));
         if (world > 1) {
             SB_TRY(sync_info(c, f));
@@ -1144,6 +1087,7 @@ int32_t cholesky_packed(sb_ctx* c, sb_factor* f, bool force_local = false) {
     };
     std::vector<int> evkind;  // kind of the interval ENDING at event i: 0 panel, 1 comm, 2 trailing(big), 3 start
     auto markk = [&](int kind) { if (ft) { mark(); evkind.push_back(kind); } };
+    std::vector<CommEv> comm_ev;
     double flops = 0;
     int64_t nlaunch = 0;
     // the OUTER_BLOCKS panels of an outer step, each in TILED layout (gemm_nt.cu); row block 0 <->
@@ -1153,23 +1097,13 @@ int32_t cholesky_packed(sb_ctx* c, sb_factor* f, bool force_local = false) {
     for (int q = 0; q < OUTER_BLOCKS; q++) Pt[q] = Pw[q] = f->panel + (int64_t)q * tiled_panel_elems(Np);
     for (int64_t k0 = 0; k0 < nblk; k0 += OUTER_BLOCKS) {
         const int nq = (int)(nblk - k0 < OUTER_BLOCKS ? nblk - k0 : OUTER_BLOCKS);
-        for (int q = 0; q < nq; q++) {
-            const int64_t kq = k0 + q;
-            const int64_t mq = Np - (kq + 1) * NB;  // rows below diagonal block kq
-            const int owner = (int)(kq % world);
-            double* Pq = Pw[q] + tiled_panel_elems((int64_t)q * NB);  // its first row block is block row kq+1
+        for (int q = 0; q < nq; q++) {   // one panel at a time: the panel work, exchange and untile are timed apart
             markk(3);
-            if (owner == rank) {
-                // bring block column kq up to date with the panels already factored in this outer step
-                if (q > 0) launch_syrk_packed(f->L, k0, Pt, q, kq, kq + 1, rank, world, st);
-                launch_potrf_inv(f->L, kq, f->N, f->invL, f->logdet_blk, f->info_dev, st, world > 1 ? f->ldiag : nullptr);
-                if (mq > 0)
-                    launch_trsm_tiled(f->L.blk(kq + 1, kq), f->L.ld(kq), f->invL + kq * (int64_t)NB * NB, Pq, mq, st);
+            SB_TRY(panel_phase(c, f, k0, q, q + 1, Pw, Pt, rank, world, st, &comm_ev));
+            if (ft) {   // the interval ending before the exchange is panel work, the exchange itself comm
+                ev.push_back(comm_ev.back().a); evkind.push_back(0);
+                ev.push_back(comm_ev.back().b); evkind.push_back(1);
             }
-            markk(0);
-            if (world > 1) SB_TRY(bcast_panel(c, f, kq, Pq, mq > 0 ? (size_t)tiled_panel_elems(mq) : 0, owner, st));
-            markk(1);
-            if (mq > 0) launch_untile_panel(Pt[q], q, mq / NB, f->L.blk(kq + 1, kq), f->L.ld(kq), st);
         }
         const int64_t jt = k0 + nq;  // first trailing block column
         if (jt < nblk) {
@@ -1226,35 +1160,17 @@ static int32_t sync_info(sb_ctx* c, sb_factor* f) {
 
 // forward sweep  b <- L^{-1} b  for S right-hand sides (b: Np x S, ld Np)
 void forward_solve(sb_ctx* c, sb_factor* f, double* b, int S) {
-    const int64_t nblk = f->L.nblk();
     for (int s0 = 0; s0 < S; s0 += 8) {
         int s = S - s0 < 8 ? S - s0 : 8;
-        double* bb = b + (int64_t)s0 * f->Np;
-        if (!c->legacy_solve) {
-            launch_sweep(f->L, f->invL, bb, s, false, f->sweep_flags, c->num_sms, c->stream, c->sweep_variant);
-            continue;
-        }
-        for (int64_t k = 0; k < nblk; k++) {
-            launch_trsv_diag(f->invL + k * (int64_t)NB * NB, bb + k * NB, f->Np, s, false, c->stream);
-            launch_gemv_below(f->L, k, bb, s, c->stream);
-        }
+        launch_sweep(f->L, f->invL, b + (int64_t)s0 * f->Np, s, false, f->sweep_flags, c->num_sms, c->stream);
     }
 }
 
 // backward sweep  b <- L^{-T} b
 void backward_solve(sb_ctx* c, sb_factor* f, double* b, int S) {
-    const int64_t nblk = f->L.nblk();
     for (int s0 = 0; s0 < S; s0 += 8) {
         int s = S - s0 < 8 ? S - s0 : 8;
-        double* bb = b + (int64_t)s0 * f->Np;
-        if (!c->legacy_solve) {
-            launch_sweep(f->L, f->invL, bb, s, true, f->sweep_flags, c->num_sms, c->stream, c->sweep_variant);
-            continue;
-        }
-        for (int64_t k = nblk - 1; k >= 0; k--) {
-            launch_gemvT_below(f->L, k, bb, s, c->stream);
-            launch_trsv_diag(f->invL + k * (int64_t)NB * NB, bb + k * NB, f->Np, s, true, c->stream);
-        }
+        launch_sweep(f->L, f->invL, b + (int64_t)s0 * f->Np, s, true, f->sweep_flags, c->num_sms, c->stream);
     }
 }
 
@@ -1298,12 +1214,7 @@ int32_t sb_ctx_create(int32_t device, sb_ctx** out) {
     const char* ft = getenv("SB_FINE_TIMING");
     if (ft && ft[0] == '0') c->fine_timing = false;
     SB_CUDA(cudaDeviceGetAttribute(&c->num_sms, cudaDevAttrMultiProcessorCount, device));
-    const char* sv = getenv("SB_SOLVE");
-    c->legacy_solve = sv && !strcmp(sv, "legacy");
-    if (sv && !strcmp(sv, "a")) c->sweep_variant = 0;
-    if (sv && !strcmp(sv, "b")) c->sweep_variant = 1;
     const char* tr = getenv("SB_TRAILING");   // "dmma" | "ozaki"
-    c->trailing_mode = SB_DEFAULT_TRAILING;
     if (tr && !strcmp(tr, "dmma")) c->trailing_mode = 0;
     if (tr && !strcmp(tr, "ozaki")) c->trailing_mode = 1;
     *out = c;
@@ -1373,7 +1284,6 @@ int32_t sb_ctx_set_option(sb_ctx* c, const char* key, int64_t value) {
         return SB_OK;
     }
     if (!strcmp(key, "fine_timing")) { c->fine_timing = value != 0; return SB_OK; }
-    if (!strcmp(key, "sweep_variant")) { c->sweep_variant = (int)value; c->legacy_solve = value < 0; return SB_OK; }
     sb::set_error(std::string("unknown option ") + key);
     return SB_ERR_INVALID;
 }
@@ -1520,29 +1430,21 @@ static int32_t factor_alloc(sb_ctx* c, int64_t N, sb_factor** out) {
             if (e == cudaSuccess) e = c->pool_alloc((void**)&f->oz_scale[i], (size_t)f->Np * sizeof(double));
             if (e == cudaSuccess) e = c->pool_alloc((void**)&f->oz_expo[i], (size_t)f->Np * sizeof(int));
         }
+        constexpr int64_t WD = (int64_t)OUTER_BLOCKS * NB;
+        if (e == cudaSuccess) e = c->pool_alloc((void**)&f->wide_D, (size_t)2 * 2 * WD * WD * sizeof(double));
+        if (e == cudaSuccess) e = c->pool_alloc((void**)&f->wide_W, (size_t)WD * WD * sizeof(double));
+        if (e == cudaSuccess) e = c->pool_alloc((void**)&f->wide_wp, oz_planes_bytes(WD));
+        if (e == cudaSuccess) e = c->pool_alloc((void**)&f->wide_wscale, (size_t)WD * sizeof(double));
+        if (e == cudaSuccess) e = c->pool_alloc((void**)&f->wide_wexpo, (size_t)WD * sizeof(int));
         if (e == cudaSuccess) {
             if (oz_make_maps(f->oz_planes[0], f->Np, &f->oz_maps[0]) != 0 ||
-                oz_make_maps(f->oz_planes[1], f->Np, &f->oz_maps[1]) != 0) {
+                oz_make_maps(f->oz_planes[1], f->Np, &f->oz_maps[1]) != 0 ||
+                oz_make_maps(f->wide_wp, WD, &f->wide_wmaps) != 0) {
                 sb_factor_destroy(f);
                 sb::set_error("cuTensorMapEncodeTiled failed for the int8 digit planes");
                 return SB_ERR_CUDA;
             }
             f->oz = true;
-            static const bool no_wide = getenv("SB_WIDE_PANEL") && getenv("SB_WIDE_PANEL")[0] == '0';
-            if (!no_wide) {
-                constexpr int64_t WD = (int64_t)OUTER_BLOCKS * NB;
-                e = c->pool_alloc((void**)&f->wide_D, (size_t)2 * 2 * WD * WD * sizeof(double));
-                if (e == cudaSuccess) e = c->pool_alloc((void**)&f->wide_W, (size_t)WD * WD * sizeof(double));
-                if (e == cudaSuccess) e = c->pool_alloc((void**)&f->wide_wp, oz_planes_bytes(WD));
-                if (e == cudaSuccess) e = c->pool_alloc((void**)&f->wide_wscale, (size_t)WD * sizeof(double));
-                if (e == cudaSuccess) e = c->pool_alloc((void**)&f->wide_wexpo, (size_t)WD * sizeof(int));
-                if (e == cudaSuccess && oz_make_maps(f->wide_wp, WD, &f->wide_wmaps) != 0) {
-                    sb_factor_destroy(f);
-                    sb::set_error("cuTensorMapEncodeTiled failed for the inv(L_512) digit planes");
-                    return SB_ERR_CUDA;
-                }
-                f->wide = e == cudaSuccess;
-            }
         }
     }
     if (e != cudaSuccess) {

@@ -50,7 +50,7 @@ struct OzArgs {
     int64_t total_tiles;
     int64_t tile_lo, tile_hi;   // this launch covers tiles [tile_lo, tile_hi) of the list (a trailing update can be split)
     int tri;             // plain mode: B is block lower triangular (128-blocks): column block q only needs K <= 128 (q + 1)
-    int tiles_per_cta;   // 0: persistent CTAs (tile t = blockIdx.x + i*gridDim.x); > 0: CTA b owns tiles [b*tpc, (b+1)*tpc)
+    int tiles_per_cta;   // always 0 (persistent CTAs); read by the tile loop, see oz_t_begin
     int kchunks;      // K / OZ_KC
     const double* scaleA;  // row scales s_i = 2^(e_i - 31), indexed by plane row of A / B
     const double* scaleB;
@@ -128,10 +128,10 @@ __device__ __forceinline__ void wgmma_s8(int (&d)[32], uint64_t da, uint64_t db)
         : "memory");
 }
 
-// Tile range of this CTA.  Persistent mode strides the whole list by gridDim.x; chunked mode gives every
-// CTA a short contiguous run and lets the CTA retire, so that kernels of a higher-priority stream (the
-// look-ahead panel phase and its NCCL broadcast) get SMs within microseconds instead of waiting for a
-// persistent grid to finish.
+// Tile range of this CTA: persistent CTAs, tile t = tile_lo + blockIdx.x + i*gridDim.x.  The tiles_per_cta branch
+// (CTA b owns tiles [b*tpc, (b+1)*tpc)) is never taken, but without it nvcc 12.9 schedules the consumer epilogue
+// of ozaki_syrk_kernel<false> differently, which measured 0.6% slower on an H100 80GB at 400 W.  Remove it together
+// with the K3' retune (DESIGN.md §8), which reschedules this kernel anyway.
 __device__ __forceinline__ int64_t oz_t_begin(const OzArgs& g) {
     return g.tile_lo + (g.tiles_per_cta > 0 ? (int64_t)blockIdx.x * g.tiles_per_cta : (int64_t)blockIdx.x);
 }
@@ -334,8 +334,7 @@ ozaki_syrk_kernel(const __grid_constant__ OzArgs g, const __grid_constant__ CUte
 
 // ---- digit planes of an operand panel ------------------------------------------------------------
 // Source: up to 4 segments of 128 columns each (K = 128 * nseg), element (row block rb, column k, row r)
-// of segment q at  base[q] + rb*rbs[q] + k*ld[q] + r  -- covers both the TILED Cholesky panels of
-// gemm_nt.cu (rbs = 128*132, ld = 132) and plain column-major panels (rbs = 128, ld = ld).
+// of segment q at  base[q] + rb*rbs[q] + k*ld[q] + r  (column-major panels: rbs = 128, ld = ld).
 // Output, for plane row i = out_row_base + rb*128 + r and byte kb = 128*q + k:
 //   plane[p][i*512 + kb]  (K-major, 512-byte pitch: the 3-D tensor the TMA box walks),
 //   scale[i] = 2^(e_i - 31),  expo[i] = e_i.
@@ -453,14 +452,6 @@ void launch_oz_slice(const OzSrc& src, int64_t rb_lo, int64_t nrb, int64_t out_r
     g_launch_count += 2;
 }
 
-// the nseg TILED panels of the Cholesky outer step at block column k0 (row block 0 <-> block row k0+1)
-OzSrc oz_src_tiled(const double* const* Pt, int nseg) {
-    OzSrc src{};
-    src.nseg = nseg;
-    for (int q = 0; q < nseg; q++) { src.base[q] = Pt[q]; src.ld[q] = NB + 4; src.rbs[q] = (int64_t)NB * (NB + 4); }
-    return src;
-}
-
 static int oz_launch(OzArgs& g, const OzMaps* mapsA, const OzMaps* mapsB, bool store, cudaStream_t s, int reserve_sms) {
     int64_t cap = g_oz_sms - reserve_sms;
     if (cap < 1) cap = 1;
@@ -468,11 +459,7 @@ static int oz_launch(OzArgs& g, const OzMaps* mapsA, const OzMaps* mapsB, bool s
     if (g.tile_lo < 0) g.tile_lo = 0;
     const int64_t ntiles = g.tile_hi - g.tile_lo;
     if (ntiles <= 0) return 0;
-    int64_t grid = ntiles < cap ? ntiles : cap;
-    if (reserve_sms < 0) {   // chunked, non-persistent: -reserve_sms tiles per CTA (see oz_t_begin)
-        g.tiles_per_cta = -reserve_sms;
-        grid = (ntiles + g.tiles_per_cta - 1) / g.tiles_per_cta;
-    }
+    const int64_t grid = ntiles < cap ? ntiles : cap;
     const CUtensorMap* ma = reinterpret_cast<const CUtensorMap*>(mapsA->a);
     const CUtensorMap* mb = reinterpret_cast<const CUtensorMap*>(mapsB->b);
     if (store) ozaki_syrk_kernel<true><<<(unsigned)grid, OZ_THREADS, OZ_SMEM, s>>>(g, *ma, *mb);

@@ -141,14 +141,10 @@ void launch_gemm_nt_seg(int nseg, const double* const* A, const int64_t* lda, co
                         double beta, cudaStream_t s);
 int64_t syrk_packed_tiles(int64_t nblk, int64_t k, int64_t jlo, int64_t jhi, int rank, int world);
 
-// vector solves on the packed factor (S right-hand sides, column-major N x S with ld = Np)
-void launch_trsv_diag(const double* invL, double* b, int64_t Np, int S, bool transpose,
-                      cudaStream_t s);
-void launch_gemv_below(Packed L, int64_t k, double* b, int S, cudaStream_t s);
-void launch_gemvT_below(Packed L, int64_t k, double* b, int S, cudaStream_t s);
-// one-launch persistent sweep (solve.cu): flags = 2*nblk unsigned scratch
+// one-launch persistent triangular sweep on the packed factor (solve.cu): S right-hand sides, column-major
+// with ld = Np; flags = 2*nblk unsigned scratch
 void launch_sweep(Packed L, const double* invL, double* b, int S, bool backward, unsigned* flags, int num_sms,
-                  cudaStream_t s, int variant = 0);
+                  cudaStream_t s);
 void launch_colsumsq(const double* v, int64_t n, int64_t ld, int S, double* out, cudaStream_t s);
 // y[M] (+)= W[M x n] * a[n]   (W column-major, ld)
 void launch_gemv_n(const double* W, int64_t ld, int64_t M, int64_t n, const double* a, double* y,
@@ -180,7 +176,6 @@ int oz_make_maps(signed char* planes, int64_t Np, OzMaps* out);
 // source panel of the slicer: up to 4 segments of 128 columns; element (row block rb, col k, row r) of
 // segment q at base[q] + rb*rbs[q] + k*ld[q] + r
 struct OzSrc { const double* base[4]; int64_t ld[4]; int64_t rbs[4]; int nseg; };
-OzSrc oz_src_tiled(const double* const* Pt, int nseg);
 void launch_oz_slice(const OzSrc& src, int64_t rb_lo, int64_t nrb, int64_t out_row_base, int64_t plane_rows,
                      double* scale, int* expo, signed char* planes, cudaStream_t s);
 int launch_syrk_ozaki(Packed A, int64_t k, int nseg, int64_t jlo, int64_t jhi, int rank, int world,

@@ -10,100 +10,6 @@ namespace {
 
 constexpr int MAXS = 8;  // right-hand sides processed per pass
 
-// b_k <- invL_kk * b_k   (or invL_kk^T * b_k); one CTA per right-hand side, 4 lanes per row
-__global__ void __launch_bounds__(4 * NB)
-trsv_diag_kernel(const double* __restrict__ invLk, double* __restrict__ bk, int64_t ldb,
-                 int transpose) {
-    __shared__ double x[NB];
-    double* b = bk + (int64_t)blockIdx.x * ldb;
-    const int i = threadIdx.x >> 2, part = threadIdx.x & 3;
-    if (threadIdx.x < NB) x[threadIdx.x] = b[threadIdx.x];
-    __syncthreads();
-    double acc = 0.0;
-    if (!transpose) {
-#pragma unroll 8
-        for (int p = part; p <= i; p += 4) acc = fma(invLk[p * NB + i], x[p], acc);
-    } else {
-#pragma unroll 8
-        for (int p = i + part; p < NB; p += 4) acc = fma(invLk[i * NB + p], x[p], acc);
-    }
-    acc += __shfl_xor_sync(0xffffffffu, acc, 1);
-    acc += __shfl_xor_sync(0xffffffffu, acc, 2);
-    if (part == 0) b[i] = acc;
-}
-
-// rows below block k:  b[r] -= sum_c L[r, k*NB + c] * x_k[c]
-// CTA = 64 rows x 4 column groups of 32 columns: 1024 CTAs at m = 64K rows, 16 loads in flight
-// per thread, so the sweep streams L at HBM speed instead of being latency-bound.
-__global__ void __launch_bounds__(256)
-gemv_below_kernel(Packed L, int64_t k, double* __restrict__ b, int S) {
-    __shared__ double xs[MAXS][NB];
-    __shared__ double red[3][MAXS][64];
-    const int64_t Np = L.Np;
-    for (int idx = threadIdx.x; idx < S * NB; idx += 256) {
-        int s = idx / NB, c = idx % NB;
-        xs[s][c] = b[(int64_t)s * Np + k * NB + c];
-    }
-    __syncthreads();
-    const int64_t ld = L.ld(k);
-    const int rl = threadIdx.x & 63, cg = threadIdx.x >> 6;
-    const int64_t lr = (int64_t)blockIdx.x * 64 + rl;  // m is a multiple of 128
-    const double* p = L.blk(k + 1, k) + lr + (int64_t)(cg * 32) * ld;
-    double acc[MAXS];
-#pragma unroll
-    for (int s = 0; s < MAXS; s++) acc[s] = 0.0;
-#pragma unroll 16
-    for (int c = 0; c < 32; c++) {
-        double l = p[(int64_t)c * ld];
-#pragma unroll
-        for (int s = 0; s < MAXS; s++)
-            if (s < S) acc[s] = fma(l, xs[s][cg * 32 + c], acc[s]);
-    }
-    if (cg > 0) {
-#pragma unroll
-        for (int s = 0; s < MAXS; s++)
-            if (s < S) red[cg - 1][s][rl] = acc[s];
-    }
-    __syncthreads();
-    if (cg == 0) {
-        int64_t r = (k + 1) * NB + lr;
-#pragma unroll
-        for (int s = 0; s < MAXS; s++)
-            if (s < S) b[(int64_t)s * Np + r] -= acc[s] + red[0][s][rl] + red[1][s][rl] + red[2][s][rl];
-    }
-}
-
-// b_k[c] -= sum_{r below} L[r, k*NB + c] * x[r]   (transposed product, atomics across CTAs)
-// CTA = 256 rows; each lane keeps its 8 x-values in registers, each warp owns 16 columns.
-constexpr int GT_ROWS = 256;
-__global__ void __launch_bounds__(256)
-gemvT_below_kernel(Packed L, int64_t k, double* __restrict__ b, int S) {
-    const int64_t Np = L.Np;
-    const int64_t ld = L.ld(k);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int64_t r0 = (int64_t)blockIdx.x * GT_ROWS;  // m is a multiple of 128; GT_ROWS | 256
-    const int64_t m = ld - NB;
-    const double* base = L.blk(k + 1, k) + r0 + lane;
-    for (int s = 0; s < S; s++) {
-        const double* x = b + (int64_t)s * Np + (k + 1) * NB + r0 + lane;
-        double xr[GT_ROWS / 32];
-#pragma unroll
-        for (int i = 0; i < GT_ROWS / 32; i++) xr[i] = (r0 + lane + 32 * i < m) ? x[32 * i] : 0.0;
-#pragma unroll 4
-        for (int cc = 0; cc < 16; cc++) {
-            int c = warp * 16 + cc;
-            const double* colp = base + (int64_t)c * ld;
-            double acc = 0.0;
-#pragma unroll
-            for (int i = 0; i < GT_ROWS / 32; i++)
-                if (r0 + lane + 32 * i < m) acc = fma(colp[32 * i], xr[i], acc);
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-            if (lane == 0) atomicAdd(&b[(int64_t)s * Np + k * NB + c], -acc);
-        }
-    }
-}
-
 // ---- persistent triangular sweep ------------------------------------------------------------
 // One launch per sweep instead of 2 launches per 128-wide block (1024 tiny dependent launches at
 // N = 65536 would leave the sweep launch-latency bound).  Right-looking data flow with static ownership:
@@ -112,11 +18,12 @@ gemvT_below_kernel(Packed L, int64_t k, double* __restrict__ b, int S) {
 //   backward b <- L^{-T} b :  when x_k = invL_kk^T b_k is final, every block j < k applies
 //                             b_j -= L[k,j]^T x_k.
 // Block i (resp. j) is owned by worker CTA (i mod W) for the whole sweep, so updates of one block
-// are sequential inside one CTA: no atomics on b, bit-reproducible results.  The owner applies the
-// last update of its block and immediately does the diagonal solve, then publishes ready[k]
-// (release/acquire; x_k is read with ld.cg on the other SMs).  The serial chain per block is
-// flag -> x_k -> one 128x128 product with L[k+1,k] -> one with invL_{k+1} -> flag, with both
-// operands prefetched into L2 before the wait.  Each element of L is read once (17.2 GB/sweep).
+// are sequential inside one CTA: no atomics on b, bit-reproducible results.  After each update the
+// owner bumps done[i]; one dedicated CTA waits until block k has all its updates, does the diagonal
+// solve and publishes ready[k] (release/acquire; x_k is read with ld.cg on the other SMs).  The serial
+// chain per block is flag -> x_k -> one 128x128 product with L[k+1,k] -> flag -> one with invL_{k+1}
+// -> flag, with each operand prefetched into L2 before the wait.  Each element of L is read once
+// (17.2 GB/sweep).
 struct SweepArgs {
     Packed L;
     const double* invL;
@@ -217,10 +124,15 @@ __device__ __forceinline__ void block_matvec_t(const double* __restrict__ M, int
     __syncthreads();
 }
 
-__device__ __forceinline__ void prefetch_block_l2(const double* M, int64_t ld);
-// variant A: dedicated CTA for the diagonal solves, done[] counters; variant B below -- owner does the
-// diagonal solve, L2 prefetch -- is the alternative (sweep_variant)
-template <bool BACKWARD, bool PF>
+__device__ __forceinline__ void prefetch_block_l2(const double* M, int64_t ld) {
+    // 128 x 128 doubles = 1024 lines of 128 B: 4 per thread
+    for (int idx = threadIdx.x; idx < 1024; idx += 256) {
+        const double* p = M + (int64_t)(idx >> 3) * ld + (idx & 7) * 16;
+        asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
+    }
+}
+
+template <bool BACKWARD>
 __global__ void __launch_bounds__(256) sweep_kernel_a(SweepArgs a) {
     __shared__ double xs[MAXS][NB];
     __shared__ double red[MAXS][NB];
@@ -262,7 +174,7 @@ __global__ void __launch_bounds__(256) sweep_kernel_a(SweepArgs a) {
         // ---- diagonal solves, in dependency order ----
         for (int64_t kk = 0; kk < nblk; kk++) {
             const int64_t k = BACKWARD ? nblk - 1 - kk : kk;
-            if (PF) prefetch_block_l2(a.invL + k * (int64_t)NB * NB, NB);
+            prefetch_block_l2(a.invL + k * (int64_t)NB * NB, NB);
             if (threadIdx.x == 0) spin_until(a.done + k, (unsigned)kk);  // all kk updates of b_k applied
             __syncthreads();
             diag_solve(k);
@@ -278,10 +190,8 @@ __global__ void __launch_bounds__(256) sweep_kernel_a(SweepArgs a) {
         int64_t first;
         if (!BACKWARD) { first = k + 1 + (((me - (k + 1)) % W) + W) % W; if (first >= nblk) continue; }
         else           { first = k - 1 - ((((k - 1) - me) % W) + W) % W; if (first < 0) continue; }
-        if (PF) {
-            if (!BACKWARD) prefetch_block_l2(a.L.blk(first, k), a.L.ld(k));
-            else prefetch_block_l2(a.L.blk(k, first), a.L.ld(first));
-        }
+        if (!BACKWARD) prefetch_block_l2(a.L.blk(first, k), a.L.ld(k));
+        else prefetch_block_l2(a.L.blk(k, first), a.L.ld(first));
         if (threadIdx.x == 0) spin_until(a.ready + k, 1u);
         __syncthreads();
         load_x(k);
@@ -294,73 +204,6 @@ __global__ void __launch_bounds__(256) sweep_kernel_a(SweepArgs a) {
             for (int64_t j = first; j >= 0; j -= W) {
                 update(j, k);
                 if (threadIdx.x == 0) { __threadfence(); red_release_add(a.done + j, 1u); }
-            }
-        }
-    }
-}
-
-__device__ __forceinline__ void prefetch_block_l2(const double* M, int64_t ld) {
-    // 128 x 128 doubles = 1024 lines of 128 B: 4 per thread
-    for (int idx = threadIdx.x; idx < 1024; idx += 256) {
-        const double* p = M + (int64_t)(idx >> 3) * ld + (idx & 7) * 16;
-        asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
-    }
-}
-
-template <bool BACKWARD, bool PF>
-__global__ void __launch_bounds__(256) sweep_kernel_b(SweepArgs a) {
-    __shared__ double xs[MAXS][NB];
-    __shared__ double red[MAXS][NB];
-    const int64_t nblk = a.L.nblk(), Np = a.L.Np;
-    const int S = a.S;
-    const int W = gridDim.x, me = blockIdx.x;
-    auto load_x = [&](int64_t k) {                 // x_k (possibly written by another SM) -> shared memory
-        for (int idx = threadIdx.x; idx < S * NB; idx += 256) {
-            const int s = idx / NB, c = idx % NB;
-            xs[s][c] = __ldcg(a.b + (int64_t)s * Np + k * NB + c);
-        }
-        __syncthreads();
-    };
-    auto diag_solve_publish = [&](int64_t k) {     // b_k is final: x_k = invL_kk b_k (or ^T), then publish
-        load_x(k);
-        const double* Mk = a.invL + k * (int64_t)NB * NB;
-        if (!BACKWARD) block_matvec_n<true>(Mk, NB, xs, a.b + k * NB, Np, S, red);
-        else block_matvec_t<true>(Mk, NB, xs, a.b + k * NB, Np, S);
-        if (threadIdx.x == 0) { __threadfence(); st_release(a.ready + k, 1u); }
-    };
-    auto update = [&](int64_t tgt, int64_t k) {   // block `tgt` absorbs x_k (already in xs)
-        if (!BACKWARD) block_matvec_n<false>(a.L.blk(tgt, k), a.L.ld(k), xs, a.b + tgt * NB, Np, S, red);
-        else block_matvec_t<false>(a.L.blk(k, tgt), a.L.ld(tgt), xs, a.b + tgt * NB, Np, S);
-    };
-
-    const int64_t kfirst = BACKWARD ? nblk - 1 : 0;
-    if ((int)(kfirst % W) == me) diag_solve_publish(kfirst);   // the first block needs no update
-
-    for (int64_t kk = 0; kk + 1 < nblk; kk++) {
-        const int64_t k = BACKWARD ? nblk - 1 - kk : kk;
-        // nearest owned target first: when it is the block next to k it gates the whole chain
-        int64_t first;
-        if (!BACKWARD) { first = k + 1 + (((me - (k + 1)) % W) + W) % W; if (first >= nblk) continue; }
-        else           { first = k - 1 - ((((k - 1) - me) % W) + W) % W; if (first < 0) continue; }
-        const bool critical = BACKWARD ? (first == k - 1) : (first == k + 1);
-        // pull the operands of the critical path into L2 BEFORE waiting for x_k
-        if (PF) {
-            if (!BACKWARD) prefetch_block_l2(a.L.blk(first, k), a.L.ld(k));
-            else prefetch_block_l2(a.L.blk(k, first), a.L.ld(first));
-            if (critical) prefetch_block_l2(a.invL + first * (int64_t)NB * NB, NB);
-        }
-        if (threadIdx.x == 0) spin_until(a.ready + k, 1u);
-        __syncthreads();
-        load_x(k);
-        if (!BACKWARD) {
-            for (int64_t i = first; i < nblk; i += W) {
-                update(i, k);
-                if (i == k + 1) { diag_solve_publish(i); load_x(k); }   // b_{k+1} just became final
-            }
-        } else {
-            for (int64_t j = first; j >= 0; j -= W) {
-                update(j, k);
-                if (j == k - 1) { diag_solve_publish(j); load_x(k); }
             }
         }
     }
@@ -562,19 +405,13 @@ __global__ void add_diag_kernel(Packed L, const double* __restrict__ d, int64_t 
 // whole forward (backward = true: transposed) sweep b <- L^{-1} b / L^{-T} b in ONE launch;
 // flags: 2*nblk unsigned scratch (zeroed here)
 void launch_sweep(Packed L, const double* invL, double* b, int S, bool backward, unsigned* flags, int num_sms,
-                  cudaStream_t s, int variant) {
+                  cudaStream_t s) {
     const int64_t nblk = L.nblk();
     cudaMemsetAsync(flags, 0, 2 * nblk * sizeof(unsigned), s);
     SweepArgs a{L, invL, b, S, flags, flags + nblk};
-    if (variant == 1 || variant == 3) {   // B: owner does the diagonal solve (1: with L2 prefetch)
-        int grid = (int)(nblk < num_sms ? nblk : num_sms);
-        if (variant == 1) { if (backward) sweep_kernel_b<true, true><<<grid, 256, 0, s>>>(a); else sweep_kernel_b<false, true><<<grid, 256, 0, s>>>(a); }
-        else              { if (backward) sweep_kernel_b<true, false><<<grid, 256, 0, s>>>(a); else sweep_kernel_b<false, false><<<grid, 256, 0, s>>>(a); }
-    } else {                              // A: dedicated diagonal-solve CTA (2: with L2 prefetch)
-        int grid = nblk < 4 ? 1 : (int)(nblk + 1 < num_sms ? nblk + 1 : num_sms);
-        if (variant == 2) { if (backward) sweep_kernel_a<true, true><<<grid, 256, 0, s>>>(a); else sweep_kernel_a<false, true><<<grid, 256, 0, s>>>(a); }
-        else              { if (backward) sweep_kernel_a<true, false><<<grid, 256, 0, s>>>(a); else sweep_kernel_a<false, false><<<grid, 256, 0, s>>>(a); }
-    }
+    const int grid = nblk < 4 ? 1 : (int)(nblk + 1 < num_sms ? nblk + 1 : num_sms);
+    if (backward) sweep_kernel_a<true><<<grid, 256, 0, s>>>(a);
+    else sweep_kernel_a<false><<<grid, 256, 0, s>>>(a);
     g_launch_count++;
 }
 
@@ -619,26 +456,6 @@ void launch_transpose(const double* in, int64_t ld_in, int64_t rows, int64_t col
 
 void launch_pack_lower(Packed L, const double* D, int64_t ld, double shift, cudaStream_t st) {
     pack_lower_kernel<<<dim3((unsigned)L.Np, (unsigned)((L.Np + 255) / 256)), 256, 0, st>>>(L, D, ld, shift);
-    g_launch_count++;
-}
-
-void launch_trsv_diag(const double* invLk, double* bk, int64_t ldb, int S, bool transpose,
-                      cudaStream_t s) {
-    trsv_diag_kernel<<<S, 4 * NB, 0, s>>>(invLk, bk, ldb, transpose ? 1 : 0);
-    g_launch_count++;
-}
-
-void launch_gemv_below(Packed L, int64_t k, double* b, int S, cudaStream_t s) {
-    int64_t m = L.ld(k) - NB;
-    if (m <= 0) return;
-    gemv_below_kernel<<<(unsigned)(m / 64), 256, 0, s>>>(L, k, b, S);
-    g_launch_count++;
-}
-
-void launch_gemvT_below(Packed L, int64_t k, double* b, int S, cudaStream_t s) {
-    int64_t m = L.ld(k) - NB;
-    if (m <= 0) return;
-    gemvT_below_kernel<<<(unsigned)((m + GT_ROWS - 1) / GT_ROWS), 256, 0, s>>>(L, k, b, S);
     g_launch_count++;
 }
 
