@@ -7,11 +7,11 @@ LAPACK / exact arithmetic and the CUDA sources can cite a runnable specification
 
   * `oz_slice`, `oz_product`      -- the int8 digit-plane ("Ozaki") product of stheno.jl_b200/csrc/ozaki.cu
                                      (oz_rowscale_kernel, oz_slice_kernel, the 7 grouped int32 accumulators);
-  * `wide_panel_factor`           -- the wide panel phase of api.cu (wide_diag_phase + launch_panel_solve_ozaki):
+  * `wide_panel_factor`           -- the wide panel phase of cholesky.cu (wide_diag_phase + launch_panel_solve_ozaki):
                                      512 x 512 diagonal block stacked over an identity, right-looking 128-block
                                      elimination, X = A inv(L_512)^T for the rows below;
   * `P2PExchangeModel`            -- the ready / ack / slot-guard protocol of the peer-to-peer column exchange
-                                     (api.cu "P2P panel exchange"), as a discrete-event model that can be driven
+                                     (p2p.cu), as a discrete-event model that can be driven
                                      with arbitrary interleavings.
 
 Only tests/ may import this module.

@@ -6,8 +6,10 @@ NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
 ARCH="-gencode arch=compute_90a,code=sm_90a"
 FLAGS="$ARCH -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-O2 -Xptxas -v"
 mkdir -p ../../build
-for f in assemble gemm_nt ozaki potrf solve api; do
+OBJS=""
+for f in assemble gemm_nt ozaki potrf solve p2p cholesky api; do
   $NVCC $FLAGS -c $f.cu -o ../../build/$f.o 2> ../../build/$f.ptxas.log || { cat ../../build/$f.ptxas.log; exit 1; }
+  OBJS="$OBJS ../../build/$f.o"
 done
-$NVCC $ARCH -shared -o ../libstheno_b200.so ../../build/assemble.o ../../build/gemm_nt.o ../../build/ozaki.o ../../build/potrf.o ../../build/solve.o ../../build/api.o -lcudart -ldl
+$NVCC $ARCH -shared -o ../libstheno_b200.so $OBJS -lcudart -ldl
 echo "built $(cd ..; pwd)/libstheno_b200.so"
