@@ -19,6 +19,10 @@ namespace {
 constexpr int TR = 128;  // tile rows   (2 per thread x 64 thread-rows)
 constexpr int TC = 32;   // tile cols   (8 per thread x 4 thread-cols)
 
+// Julia's max(d, 0): a NaN distance (NaN input) stays NaN, where fmax would return 0 and make a NaN input
+// look like a coincident point.
+__device__ __forceinline__ double clamp0(double d) { return d < 0.0 ? 0.0 : d; }
+
 // Distances.jl SqEuclidean pairwise: max(|x|^2 + |y|^2 - 2 x.y, 0).  For dim == 1 every
 // operation is a single correctly-rounded IEEE op in the reference's order (no FMA
 // contraction), so the result is bit-identical to the CPU path.
@@ -27,7 +31,7 @@ __device__ __forceinline__ double sqdist_gemm_trick(const double* __restrict__ x
     if (dim == 1) {
         double a = x[0], b = y[0];
         double s = __dadd_rn(__dmul_rn(a, a), __dmul_rn(b, b));
-        return fmax(__dsub_rn(s, __dmul_rn(2.0, __dmul_rn(a, b))), 0.0);
+        return clamp0(__dsub_rn(s, __dmul_rn(2.0, __dmul_rn(a, b))));
     }
     double sa = 0.0, sb_ = 0.0, dot = 0.0;
     for (int d = 0; d < dim; d++) {
@@ -35,7 +39,7 @@ __device__ __forceinline__ double sqdist_gemm_trick(const double* __restrict__ x
         sb_ = __dadd_rn(sb_, __dmul_rn(y[d], y[d]));
         dot = fma(x[d], y[d], dot);
     }
-    return fmax(__dsub_rn(__dadd_rn(sa, sb_), __dmul_rn(2.0, dot)), 0.0);
+    return clamp0(__dsub_rn(__dadd_rn(sa, sb_), __dmul_rn(2.0, dot)));
 }
 
 // Distances.colwise(SqEuclidean): direct differences (kernelmatrix_diag path).
@@ -121,8 +125,8 @@ __device__ __forceinline__ void strip_1d(const TermDev& t, double xa, double xb,
         } else {
             // Distances.jl GEMM-trick rounding sequence, op for op (no FMA contraction)
             const double y2 = __dmul_rn(y, y);
-            const double da = fmax(__dsub_rn(__dadd_rn(xa2, y2), __dmul_rn(2.0, __dmul_rn(xa, y))), 0.0);
-            const double db = fmax(__dsub_rn(__dadd_rn(xb2, y2), __dmul_rn(2.0, __dmul_rn(xb, y))), 0.0);
+            const double da = clamp0(__dsub_rn(__dadd_rn(xa2, y2), __dmul_rn(2.0, __dmul_rn(xa, y))));
+            const double db = clamp0(__dsub_rn(__dadd_rn(xb2, y2), __dmul_rn(2.0, __dmul_rn(xb, y))));
             ka = kappa(KERNEL, da, t.param);
             kb = kappa(KERNEL, db, t.param);
         }

@@ -181,7 +181,11 @@ static int32_t wide_diag_phase(sb_ctx* c, sb_factor* f, int64_t k0, int nq, int 
     launch_transpose(X + WIDE, ldd, WIDE, WIDE, f->wide_W, WIDE, st);
     OzSrc ws{};
     ws.nseg = OUTER_BLOCKS;
-    for (int q = 0; q < OUTER_BLOCKS; q++) { ws.base[q] = f->wide_W + (int64_t)q * NB * WIDE; ws.ld[q] = WIDE; ws.rbs[q] = NB; }
+    for (int q = 0; q < OUTER_BLOCKS; q++) {
+        ws.base[q] = f->wide_W + (int64_t)q * NB * WIDE; ws.ld[q] = WIDE; ws.rbs[q] = NB;
+        ws.diag[q] = f->L.blk(k0 + q, k0 + q); ws.dld[q] = f->L.ld(k0 + q);
+    }
+    ws.colsign = +1;   // column k of inv(L_512) times 2^ilogb(L_kk): see wide_bulk_phase
     launch_oz_slice(ws, 0, OUTER_BLOCKS, 0, WIDE, f->wide_wscale, f->wide_wexpo, f->wide_wp, st);
     return SB_OK;
 }
@@ -202,8 +206,14 @@ static int32_t wide_bulk_phase(sb_ctx* c, sb_factor* f, int64_t k0, int nq, int 
     for (int q = 0; q < OUTER_BLOCKS; q++) {
         xcol[q] = f->L.blk(r0, k0 + q); ldx[q] = f->L.ld(k0 + q);
         as.base[q] = xcol[q]; as.ld[q] = ldx[q]; as.rbs[q] = NB;
+        as.diag[q] = f->L.blk(k0 + q, k0 + q); as.dld[q] = f->L.ld(k0 + q);
     }
+    // Equilibrated panel solve: X = (A21 E^-1)(inv(L_512) E)^T with E = diag(2^ilogb(L_kk)).  A21[i, k] is of the
+    // order of L21[i, k] L_kk, so without E the digit planes of a row would span the range of the step's diagonal
+    // (for a diagonally scaled matrix D A D up to 2^60), and the small entries would lose their digits.
+    as.colsign = -1;
     launch_oz_slice(as, 0, below, r0 * NB, Np, f->oz_scale[set], f->oz_expo[set], f->oz_planes[set], st);
+    as.colsign = 0;    // the planes of X = L21 for the trailing update: rows only
     if (launch_panel_solve_ozaki(xcol, ldx, below * NB, &f->oz_maps[set], f->oz_scale[set], r0 * NB, &f->wide_wmaps,
                                  f->wide_wscale, st) != 0) {
         sb::set_error("int8 Ozaki panel solve failed to launch");

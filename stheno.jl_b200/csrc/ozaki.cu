@@ -22,6 +22,8 @@
 // then C -= s_i s_j acc on the packed fp64 matrix.
 // Replaces the dsyrk/dgemm inside LAPACK dpotrf (AbstractGPs `cholesky(Symmetric(cov(fx)))`).
 #include <cuda.h>
+#include <float.h>
+#include <math_constants.h>
 
 #include "sb_common.cuh"
 
@@ -338,6 +340,17 @@ ozaki_syrk_kernel(const __grid_constant__ OzArgs g, const __grid_constant__ CUte
 // Output, for plane row i = out_row_base + rb*128 + r and byte kb = 128*q + k:
 //   plane[p][i*512 + kb]  (K-major, 512-byte pitch: the 3-D tensor the TMA box walks),
 //   scale[i] = 2^(e_i - 31),  expo[i] = e_i.
+// x scaled by the power of two of its column (OzSrc column equilibration); the identity without it
+template <bool COLSCALE>
+__device__ __forceinline__ double oz_col(const OzSrc& src, int q, int k, double x) {
+    if constexpr (COLSCALE) {
+        const double d = src.diag[q][(int64_t)k * src.dld[q] + k];
+        if (d > 0.0 && d <= DBL_MAX) x = scalbn(x, src.colsign * ilogb(d));   // exact: a power of two
+    }
+    return x;
+}
+
+template <bool COLSCALE>
 __global__ void __launch_bounds__(512)
 oz_rowscale_kernel(const OzSrc src, int64_t rb_lo, int64_t out_row_base, double* __restrict__ scale,
                    int* __restrict__ expo) {
@@ -349,20 +362,28 @@ oz_rowscale_kernel(const OzSrc src, int64_t rb_lo, int64_t out_row_base, double*
     for (int q = 0; q < src.nseg; q++) {
         const double* P = src.base[q] + rb * src.rbs[q] + r;
         const int64_t ld = src.ld[q];
-        for (int k = cg; k < NB; k += 4) m = fmax(m, fabs(P[(int64_t)k * ld]));
+        for (int k = cg; k < NB; k += 4) {
+            const double a = fabs(oz_col<COLSCALE>(src, q, k, P[(int64_t)k * ld]));
+            m = fmax(m, a);
+            if (!(a <= DBL_MAX)) m = CUDART_INF;   // NaN or Inf: fmax would drop a NaN
+        }
     }
     red[cg][r] = m;
     __syncthreads();
     if (cg == 0) {
         m = fmax(fmax(red[0][r], red[1][r]), fmax(red[2][r], red[3][r]));
         const int64_t i = out_row_base + rb * NB + r;
+        // Rows with no entry above 1e-280 are zero rows: no digits, scale 0.  Rows with a NaN, an Inf or an entry of
+        // 1e280 or more cannot be cut into digits: no digits either, but scale NaN, so every product that touches the
+        // row is NaN (NaN * 0) and the pivot check reports the failure instead of factoring a zeroed row.
         const bool ok = m > 1e-280 && m < 1e280;
         const int e = ok ? ilogb(m) + 2 : 0;   // |x| * 2^-e < 0.5
-        scale[i] = ok ? scalbn(1.0, e - 31) : 0.0;
+        scale[i] = ok ? scalbn(1.0, e - 31) : (m >= 1e280 ? CUDART_NAN : 0.0);
         expo[i] = ok ? e : 0x7fffffff;
     }
 }
 
+template <bool COLSCALE>
 __global__ void __launch_bounds__(256)
 oz_slice_kernel(const OzSrc src, int64_t rb_lo, int64_t out_row_base, int64_t plane_rows,
                 const int* __restrict__ expo, signed char* __restrict__ planes) {
@@ -377,7 +398,7 @@ oz_slice_kernel(const OzSrc src, int64_t rb_lo, int64_t out_row_base, int64_t pl
     const double* P = src.base[q] + rb * src.rbs[q] + (int64_t)(kc * 32 + kh * 16) * ld + r;
 #pragma unroll 4
     for (int kk = 0; kk < 16; kk++) {
-        const double x = P[(int64_t)kk * ld];
+        const double x = oz_col<COLSCALE>(src, q, kc * 32 + kh * 16 + kk, P[(int64_t)kk * ld]);
         long long Z = 0x0000808080808080LL;
         if (e != 0x7fffffff) Z += __double2ll_rn(scalbn(x, 55 - e));
         const int kb = kh * 16 + kk;
@@ -446,9 +467,14 @@ int oz_make_maps(signed char* planes, int64_t Np, OzMaps* out) {
 void launch_oz_slice(const OzSrc& src, int64_t rb_lo, int64_t nrb, int64_t out_row_base, int64_t plane_rows,
                      double* scale, int* expo, signed char* planes, cudaStream_t s) {
     if (nrb <= 0 || src.nseg <= 0) return;
-    oz_rowscale_kernel<<<(unsigned)nrb, 512, 0, s>>>(src, rb_lo, out_row_base, scale, expo);
-    oz_slice_kernel<<<dim3((unsigned)nrb, (unsigned)(src.nseg * 4)), 256, 0, s>>>(src, rb_lo, out_row_base, plane_rows,
-                                                                                  expo, planes);
+    const dim3 grid((unsigned)nrb, (unsigned)(src.nseg * 4));
+    if (src.colsign != 0) {
+        oz_rowscale_kernel<true><<<(unsigned)nrb, 512, 0, s>>>(src, rb_lo, out_row_base, scale, expo);
+        oz_slice_kernel<true><<<grid, 256, 0, s>>>(src, rb_lo, out_row_base, plane_rows, expo, planes);
+    } else {
+        oz_rowscale_kernel<false><<<(unsigned)nrb, 512, 0, s>>>(src, rb_lo, out_row_base, scale, expo);
+        oz_slice_kernel<false><<<grid, 256, 0, s>>>(src, rb_lo, out_row_base, plane_rows, expo, planes);
+    }
     g_launch_count += 2;
 }
 

@@ -174,8 +174,15 @@ struct alignas(64) OzMaps { unsigned char a[128]; unsigned char b[128]; };  // C
 size_t oz_planes_bytes(int64_t Np);                       // 7 digit planes, 512-byte row pitch
 int oz_make_maps(signed char* planes, int64_t Np, OzMaps* out);
 // source panel of the slicer: up to 4 segments of 128 columns; element (row block rb, col k, row r) of
-// segment q at base[q] + rb*rbs[q] + k*ld[q] + r
-struct OzSrc { const double* base[4]; int64_t ld[4]; int64_t rbs[4]; int nseg; };
+// segment q at base[q] + rb*rbs[q] + k*ld[q] + r.
+// Column equilibration (colsign = -1 or +1, 0 = off): column k of segment q is multiplied by 2^(colsign * e),
+// e = ilogb of the diagonal entry  diag[q][k * dld[q] + k]  (the step's L_kk).  The panel solve scales the columns
+// of A21 by 2^-e and the same columns of inv(L_512) by 2^+e: the product is unchanged, and the digit planes of a row
+// no longer span the range of the diagonal.
+struct OzSrc {
+    const double* base[4]; int64_t ld[4]; int64_t rbs[4]; int nseg;
+    const double* diag[4]; int64_t dld[4]; int colsign;
+};
 void launch_oz_slice(const OzSrc& src, int64_t rb_lo, int64_t nrb, int64_t out_row_base, int64_t plane_rows,
                      double* scale, int* expo, signed char* planes, cudaStream_t s);
 int launch_syrk_ozaki(Packed A, int64_t k, int nseg, int64_t jlo, int64_t jhi, int rank, int world,
