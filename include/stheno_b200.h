@@ -246,6 +246,15 @@ int32_t sb_factor_get_L(sb_ctx* ctx, sb_factor* f, void* L_out);
 int32_t sb_vfe_create(sb_ctx* ctx, const sb_covspec* uu, const sb_noise* noise_u,
                       const sb_covspec* xu, const sb_covspec* ff_diag, const sb_noise* noise_f,
                       const void* delta, sb_vfe** out, double* out2, int64_t* info);
+/* sb_vfe_grad: gradient of the elbo of handle v (reverse mode of AbstractGPs elbo(VFE(fz), fx, y),
+ * src/gp/sparse_finite_gp.jl:52-58).  uu, xu, ff_diag, noise_f and delta are the ones v was created from
+ * (N and M must match the handle, noise_f diagonal and > 0).
+ * g_uu / g_xu / g_ff: 2 * nterms of each spec, [2t] = d/d coeff_t, [2t+1] = d/d log(input scale_t).
+ * g_noise_u_diag[M] = d/d (K_uu + jitter)_ii,  g_noise_f_diag[N] = d/d Sigma_y[i,i].
+ * The K_fu chunks of sb_vfe_create are streamed again (sharded over ranks, one all-reduce). */
+int32_t sb_vfe_grad(sb_ctx* ctx, sb_vfe* v, const sb_covspec* uu, const sb_covspec* xu,
+                    const sb_covspec* ff_diag, const sb_noise* noise_f, const void* delta,
+                    double* g_uu, double* g_xu, double* g_ff, void* g_noise_u_diag, void* g_noise_f_diag);
 int32_t sb_vfe_predict(sb_ctx* ctx, sb_vfe* v, const sb_covspec* cross /* N* x M */,
                        const sb_covspec* prior_diag, void* mean_out, void* var_out);
 /* sb_vfe_predict_cov replaces  cov(f_approx_post(x*)) = K** - B'B + (L_Lambda^{-1}B)'(L_Lambda^{-1}B)

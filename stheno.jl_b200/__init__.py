@@ -15,6 +15,6 @@ from .gp import (  # noqa: F401
 )
 from .finite import (  # noqa: F401
     ApproxPosteriorGP, FiniteGP, PosteriorGP, SparseFiniteGP, VFE, approx_posterior, cov, dtc, elbo,
-    LogpdfGradient, grad_logpdf, load_factor, logpdf, marginals, mean, mean_and_cov, mean_and_var, posterior, rand, save_factor, var,
+    ElboGradient, LogpdfGradient, grad_elbo, grad_logpdf, load_factor, logpdf, marginals, mean, mean_and_cov, mean_and_var, posterior, rand, save_factor, var,
 )
 from .lib import Context, PosDefException, SthenoB200Error, default_context, set_default_context  # noqa: F401

@@ -987,13 +987,15 @@ struct sb_vfe {
     std::unique_ptr<sb_factor> fu;  // chol(K_uu + jitter)
     std::unique_ptr<sb_factor> fl;  // chol(A A^T + I)
     DevArray<double> alpha{ctx};    // Mp, K_*u alpha = posterior mean
-    int64_t M = 0, Mp = 0;
+    int64_t N = 0, M = 0, Mp = 0;
     explicit sb_vfe(sb_ctx* c) : ctx(c) {}
     ~sb_vfe() {   // release order fu, fl, alpha (see ~sb_factor)
         fu.reset();
         fl.reset();
     }
 };
+
+constexpr int64_t VFE_CHUNK_ROWS = 16384;  // observation rows per chunk of the K_fu stream
 
 int32_t sb_vfe_destroy(sb_vfe* v) {
     if (!v) return SB_OK;
@@ -1025,6 +1027,7 @@ int32_t sb_vfe_create(sb_ctx* c, const sb_covspec* uu, const sb_noise* noise_u, 
     SB_TRY(factor_create_impl(c, uu, noise_u, v->fu, info, /*force_local=*/true));
     cudaEvent_t t0 = c->next_event(), t1 = c->next_event();
     cudaEventRecord(t0, c->stream);
+    v->N = N;
     v->M = M;
     v->Mp = v->fu->Np;
     const int64_t Mp = v->Mp;
@@ -1051,7 +1054,7 @@ int32_t sb_vfe_create(sb_ctx* c, const sb_covspec* uu, const sb_noise* noise_u, 
     SB_TRY(dff.build(ff_diag, c->stream, true));
     const std::vector<BlockDev> all_blocks = dxu.blocks;
 
-    const int64_t NC = 16384;  // observation rows per chunk
+    const int64_t NC = VFE_CHUNK_ROWS;
     DevBuf dsinv(c), ddt(c), W(c), T(c), Xk(c), D(c), vv(c), fro(c), varf(c);
     const int64_t nchunks_total = (N + NC - 1) / NC;
     SB_TRY(dsinv.alloc(N * sizeof(double)));
@@ -1132,6 +1135,147 @@ int32_t sb_vfe_create(sb_ctx* c, const sb_covspec* uu, const sb_noise* noise_u, 
     c->tm.total_ms += ms;
     count_launches(c, before);
     *out = v.release();
+    return SB_OK;
+}
+
+// Gradient of the elbo (reverse mode of sb_vfe_create; DESIGN.md §4).  With A = L_u^{-1} K_uf Sigma^{-1/2},
+// B = A A' + I = L_B L_B', D = B - I, alpha the handle's posterior weights, beta = Sigma^{-1}(delta - K_fu alpha)
+// and E = (I - B^{-1}) L_u^{-1}, the elbo's partial derivatives are
+//   d/dK_fu = beta alpha' + Sigma^{-1/2} A' E              (N x M: streamed in the chunks of sb_vfe_create)
+//   d/dK_uu = -(alpha alpha' + L_u^{-T} D E) / 2            (M x M: formed once)
+//   d/dK_ff[i,i] = -1 / (2 sigma_i^2)
+//   d/dsigma_i^2 = (beta_i^2 - (1 - |L_B^{-1} a_i|^2) / sigma_i^2) / 2 + (k_ii - sigma_i^2 |a_i|^2) / (2 sigma_i^4)
+// and every term of the three specs is reduced against its weight as in sb_logpdf_grad.  Multi-GPU: the chunk
+// parts (xu, ff_diag, observation noise) are partial sums over the chunks a rank owns, combined by one
+// all-reduce; the M x M part is replicated.
+int32_t sb_vfe_grad(sb_ctx* c, sb_vfe* v, const sb_covspec* uu, const sb_covspec* xu, const sb_covspec* ff_diag,
+                    const sb_noise* noise_f, const void* delta, double* g_uu, double* g_xu, double* g_ff,
+                    void* g_noise_u_diag, void* g_noise_f_diag) {
+    SB_CHECK(c && v && uu && xu && ff_diag && noise_f && delta && g_uu && g_xu && g_ff && g_noise_u_diag &&
+             g_noise_f_diag, "null argument");
+    const int64_t N = v->N, M = v->M, Mp = v->Mp;
+    SB_CHECK(xu->nrows == N && xu->ncols == M, "xu must be the N x M spec the handle was created from");
+    SB_CHECK(uu->nrows == M && uu->ncols == M && uu->symmetric == 1, "uu must be the symmetric M x M spec of cov(fz)");
+    SB_CHECK(ff_diag->nrows == N && ff_diag->ncols == N, "ff_diag must be the N x N diag spec of var(f, x)");
+    SB_CHECK(noise_f->dense == nullptr, "VFE needs diagonal observation noise");
+    begin_call(c);
+    int64_t before = g_launch_count;
+    cudaEvent_t t0 = c->next_event(), t1 = c->next_event();
+    cudaEventRecord(t0, c->stream);
+
+    // host O(N) prep: [delta | sigma^2 | sigma^-1 | d elbo / d K_ff[i,i]]
+    std::vector<double> hobs(4 * N);
+    double* hd = hobs.data();
+    double* hs2 = hd + N;
+    SB_CUDA(cudaMemcpy(hd, delta, N * sizeof(double), cudaMemcpyDefault));
+    if (noise_f->diag) SB_CUDA(cudaMemcpy(hs2, noise_f->diag, N * sizeof(double), cudaMemcpyDefault));
+    else for (int64_t i = 0; i < N; i++) hs2[i] = noise_f->sigma2;
+    for (int64_t i = 0; i < N; i++) {
+        SB_CHECK(hs2[i] > 0.0, "VFE needs positive observation noise");
+        hd[2 * N + i] = 1.0 / sqrt(hs2[i]);
+        hd[3 * N + i] = -0.5 / hs2[i];
+    }
+
+    DevSpec duu(c), dxu(c), dff(c);
+    SB_TRY(duu.build(uu, c->stream, false));
+    SB_TRY(dxu.build(xu, c->stream, false));
+    SB_TRY(dff.build(ff_diag, c->stream, true));
+    const std::vector<BlockDev> xu_blocks = dxu.blocks, ff_blocks = dff.blocks;
+    const int64_t NC = VFE_CHUNK_ROWS < round_up(N, NB) ? VFE_CHUNK_ROWS : round_up(N, NB);
+    const int64_t nchunks_total = (N + VFE_CHUNK_ROWS - 1) / VFE_CHUNK_ROWS;
+    const int64_t nuu = 2 * (int64_t)uu->nterms, nxu = 2 * (int64_t)xu->nterms, nff = 2 * (int64_t)ff_diag->nterms;
+    const size_t mm = (size_t)Mp * Mp;
+    DevBuf obs(c), part(c), guu(c), gnu(c), Wu(c), Et(c), A1(c), A2(c), W(c), S(c), Xk(c), cv(c);
+    SB_TRY(obs.alloc(4 * N * sizeof(double)));
+    SB_TRY(part.alloc((nxu + nff + N) * sizeof(double)));   // chunk partial sums: [g_xu | g_ff | g_noise_f]
+    SB_TRY(guu.alloc((nuu > 0 ? nuu : 1) * sizeof(double)));
+    SB_TRY(gnu.alloc(Mp * sizeof(double)));
+    for (DevBuf* b : {&Wu, &Et, &A1, &A2}) SB_TRY(b->alloc(mm * sizeof(double)));
+    SB_TRY(W.alloc((size_t)NC * Mp * sizeof(double)));
+    SB_TRY(S.alloc((size_t)NC * Mp * sizeof(double)));
+    SB_TRY(Xk.alloc((size_t)(NC > Mp ? NC : Mp) * SWEEP_COLS * sizeof(double)));
+    SB_TRY(cv.alloc((size_t)5 * NC * sizeof(double)));
+    const double* d_delta = obs.d();
+    const double* d_s2 = obs.d() + N;
+    const double* d_sinv = obs.d() + 2 * N;
+    const double* d_wff = obs.d() + 3 * N;
+    double* g_part_xu = part.d();
+    double* g_part_ff = part.d() + nxu;
+    double* g_part_nf = part.d() + nxu + nff;
+    double* t = cv.d();
+    double* beta = cv.d() + NC;
+    double* la = cv.d() + 2 * NC;
+    double* lb = cv.d() + 3 * NC;
+    double* kff = cv.d() + 4 * NC;
+    SB_CUDA(cudaMemcpyAsync(obs.p, hobs.data(), 4 * N * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+    SB_CUDA(cudaMemsetAsync(part.p, 0, part.bytes, c->stream));
+    SB_CUDA(cudaMemsetAsync(guu.p, 0, guu.bytes, c->stream));
+
+    // M^3 prologue (DMMA sweeps and products): E^T = L_u^{-T} (I - B^{-1}) and P = L_u^{-T} D E
+    for (DevBuf* b : {&Wu, &A1, &A2}) SB_CUDA(cudaMemsetAsync(b->p, 0, mm * sizeof(double), c->stream));
+    launch_set_scaled_identity(Wu.d(), Mp, 1.0, c->stream);
+    launch_set_scaled_identity(A1.d(), Mp, 1.0, c->stream);
+    launch_set_scaled_identity(A2.d(), Mp, 1.0, c->stream);
+    SB_TRY(trsm_sweep(c, v->fu.get(), Wu.d(), Mp, Xk.d(), /*keep=*/true, nullptr));         // Wu = L_u^{-T}
+    SB_TRY(trsm_sweep(c, v->fl.get(), A1.d(), Mp, Xk.d(), /*keep=*/true, nullptr));         // A1 = L_B^{-T}
+    launch_gemm_nt(A1.d(), Mp, A1.d(), Mp, A2.d(), Mp, Mp, Mp, Mp, -1.0, 1.0, c->stream);  // A2 = I - B^{-1}
+    launch_gemm_nt(Wu.d(), Mp, A2.d(), Mp, Et.d(), Mp, Mp, Mp, Mp, 1.0, 0.0, c->stream);   // E^T
+    launch_unpack_lower(v->fl->L, Mp, A1.d(), c->stream);                                  // A1 = L_B
+    SB_CUDA(cudaMemsetAsync(A2.p, 0, mm * sizeof(double), c->stream));
+    launch_set_scaled_identity(A2.d(), Mp, -1.0, c->stream);
+    launch_gemm_nt(A1.d(), Mp, A1.d(), Mp, A2.d(), Mp, Mp, Mp, Mp, 1.0, 1.0, c->stream);   // A2 = D
+    launch_gemm_nt(Wu.d(), Mp, A2.d(), Mp, A1.d(), Mp, Mp, Mp, Mp, 1.0, 0.0, c->stream);   // A1 = L_u^{-T} D
+    launch_gemm_nt(A1.d(), Mp, Et.d(), Mp, A2.d(), Mp, Mp, Mp, Mp, 1.0, 0.0, c->stream);   // A2 = P
+    for (auto& b : duu.blocks) {
+        const bool offdiag = b.row0 != b.col0;   // symmetric spec: (i, j), j < i, stands for (j, i) too
+        launch_grad_reduce_outer(b, -0.5, v->alpha, v->alpha, -0.5, A2.d(), Mp, offdiag ? 2.0 : 1.0, guu.d(), c->stream);
+    }
+    launch_vfe_uu_diag(v->alpha, A2.d(), Mp, M, gnu.d(), c->stream);
+    SB_CUDA(cudaGetLastError());
+
+    // the observation stream: the chunks of sb_vfe_create, round-robin over ranks
+    OzSweepWs ws(c);
+    if (v->fu->oz || v->fl->oz) SB_TRY(ws.init(NC));
+    for (int64_t ci = c->rank; ci < nchunks_total; ci += c->world) {
+        const int64_t r0 = ci * VFE_CHUNK_ROWS, r1 = r0 + VFE_CHUNK_ROWS < N ? r0 + VFE_CHUNK_ROWS : N;
+        const int64_t rows = r1 - r0, rows_p = round_up(rows, NB);
+        dxu.blocks = xu_blocks;
+        dxu.nrows = N;
+        clip_rows(dxu, r0, r1, false);
+        dff.blocks = ff_blocks;
+        dff.nrows = dff.ncols = N;
+        clip_rows(dff, r0, r1, true);
+        SB_CUDA(cudaMemsetAsync(W.p, 0, (size_t)rows_p * Mp * sizeof(double), c->stream));
+        SB_CUDA(cudaMemsetAsync(la, 0, 2 * NC * sizeof(double), c->stream));   // la, lb
+        SB_CUDA(cudaMemsetAsync(kff, 0, NC * sizeof(double), c->stream));
+        SB_TRY(assemble_dense(c, dxu, W.d(), rows_p));                                        // K_fu rows
+        launch_gemv_n(W.d(), rows_p, rows_p, Mp, v->alpha, t, c->stream);                    // t = K_fu alpha
+        launch_vfe_beta(d_delta + r0, t, d_s2 + r0, rows, rows_p, beta, c->stream);
+        launch_rowscale(W.d(), rows_p, rows, Mp, d_sinv + r0, c->stream);
+        SB_TRY(trsm_sweep(c, v->fu.get(), W.d(), rows_p, Xk.d(), /*keep=*/true, la, &ws));  // A' rows, |a_i|^2
+        launch_gemm_nt(W.d(), rows_p, Et.d(), Mp, S.d(), rows_p, rows_p, Mp, Mp, 1.0, 0.0, c->stream);
+        launch_rowscale(S.d(), rows_p, rows, Mp, d_sinv + r0, c->stream);                    // S = Sigma^{-1/2} A' E
+        for (auto& b : dxu.blocks)
+            launch_grad_reduce_outer(b, 1.0, beta, v->alpha, 1.0, S.d(), rows_p, 1.0, g_part_xu, c->stream);
+        SB_TRY(assemble_diag(c, dff, kff));
+        for (auto& b : dff.blocks) launch_grad_diag(b, d_wff + r0, g_part_ff, c->stream);
+        SB_TRY(trsm_sweep(c, v->fl.get(), W.d(), rows_p, Xk.d(), /*keep=*/false, lb, &ws)); // |L_B^{-1} a_i|^2
+        launch_vfe_noise_grad(beta, la, lb, kff, d_s2 + r0, rows, g_part_nf + r0, c->stream);
+    }
+    SB_CUDA(cudaGetLastError());
+    if (c->world > 1)
+        SB_NCCL(nccl_dl::AllReduce(part.p, part.p, (size_t)(nxu + nff + N), ncclDouble, ncclSum, c->comm, c->stream));
+    if (nuu > 0) SB_CUDA(cudaMemcpyAsync(g_uu, guu.p, nuu * sizeof(double), cudaMemcpyDefault, c->stream));
+    if (nxu > 0) SB_CUDA(cudaMemcpyAsync(g_xu, g_part_xu, nxu * sizeof(double), cudaMemcpyDefault, c->stream));
+    if (nff > 0) SB_CUDA(cudaMemcpyAsync(g_ff, g_part_ff, nff * sizeof(double), cudaMemcpyDefault, c->stream));
+    SB_CUDA(cudaMemcpyAsync(g_noise_u_diag, gnu.p, M * sizeof(double), cudaMemcpyDefault, c->stream));
+    SB_CUDA(cudaMemcpyAsync(g_noise_f_diag, g_part_nf, N * sizeof(double), cudaMemcpyDefault, c->stream));
+    cudaEventRecord(t1, c->stream);
+    SB_CUDA(cudaStreamSynchronize(c->stream));
+    float ms = 0;
+    cudaEventElapsedTime(&ms, t0, t1);
+    c->tm.total_ms += ms;
+    count_launches(c, before);
     return SB_OK;
 }
 

@@ -269,9 +269,34 @@ __device__ __forceinline__ void kappa_and_dlogs(int kernel, double d2, double pa
     }
 }
 
+// weight Q_rc of the logpdf gradient: (alpha_r alpha_c - Kinv_rc) / 2
+struct LogpdfWeight {
+    const double* __restrict__ alpha;
+    const double* __restrict__ Kinv;
+    int64_t ld;
+    __device__ __forceinline__ double row(int64_t r) const { return alpha[r]; }
+    __device__ __forceinline__ double operator()(double ar, int64_t r, int64_t c) const {
+        return 0.5 * (ar * alpha[c] - Kinv[c * ld + r]);
+    }
+};
+
+// weight Q_rc = a u_r v_c + b G_rc of the elbo gradient (G dense column-major, ld)
+struct OuterPlusDense {
+    double a;
+    const double* __restrict__ u;
+    const double* __restrict__ v;
+    double b;
+    const double* __restrict__ G;
+    int64_t ld;
+    __device__ __forceinline__ double row(int64_t r) const { return a * u[r]; }
+    __device__ __forceinline__ double operator()(double aur, int64_t r, int64_t c) const {
+        return aur * v[c] + b * G[c * ld + r];
+    }
+};
+
+template <class Weight>
 __global__ void __launch_bounds__(256)
-grad_reduce_kernel(const __grid_constant__ BlockDev b, const double* __restrict__ alpha,
-                   const double* __restrict__ Kinv, int64_t ld, double w, double* __restrict__ g) {
+grad_reduce_kernel(const __grid_constant__ BlockDev b, const Weight wt, double w, double* __restrict__ g) {
     // tile 64 rows x 32 cols; thread: 1 row x 8 cols
     const int64_t r = b.row0 + (int64_t)blockIdx.x * 64 + (threadIdx.x & 63);
     const int64_t c0 = b.col0 + (int64_t)blockIdx.y * 32 + (threadIdx.x >> 6) * 8;
@@ -279,11 +304,11 @@ grad_reduce_kernel(const __grid_constant__ BlockDev b, const double* __restrict_
 #pragma unroll
     for (int t = 0; t < MAX_TERMS; t++) acc[t][0] = acc[t][1] = 0.0;
     if (r < b.row0 + b.nrows) {
-        const double ar = alpha[r];
+        const double ar = wt.row(r);
         for (int j = 0; j < 8; j++) {
             const int64_t c = c0 + j;
             if (c >= b.col0 + b.ncols) break;
-            const double q = 0.5 * (ar * alpha[c] - Kinv[c * ld + r]);
+            const double q = wt(ar, r, c);
             for (int ti = 0; ti < b.nterms; ti++) {
                 const TermDev& t = b.t[ti];
                 const double* x = t.zl + (r - b.row0) * t.dim;
@@ -314,6 +339,48 @@ grad_reduce_kernel(const __grid_constant__ BlockDev b, const double* __restrict_
         double v = 0.0;
         for (int wdx = 0; wdx < 8; wdx++) v += red[wdx][ti][h];
         atomicAdd(&g[2 * b.tix[ti] + h], w * v);
+    }
+}
+
+// the same two sums over the paired points of a diag spec: point i of the block carries the weight
+// wdiag[row0 + i] (elbo: d/d K_ff[i, i] = -1 / (2 sigma_i^2))
+__global__ void __launch_bounds__(256)
+grad_diag_kernel(const __grid_constant__ BlockDev b, const double* __restrict__ wdiag, double* __restrict__ g) {
+    const int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x;
+    double acc[MAX_TERMS][2];
+#pragma unroll
+    for (int t = 0; t < MAX_TERMS; t++) acc[t][0] = acc[t][1] = 0.0;
+    if (i < b.nrows) {
+        const double q = wdiag[b.row0 + i];
+        for (int ti = 0; ti < b.nterms; ti++) {
+            const TermDev& t = b.t[ti];
+            const double* x = t.zl + i * t.dim;
+            const double* y = t.zr + i * t.dim;
+            double k, dk;
+            if (t.kernel == SB_K_WHITE) { k = all_equal(x, y, t.dim) ? 1.0 : 0.0; dk = 0.0; }
+            else kappa_and_dlogs(t.kernel, sqdist_direct(x, y, t.dim), t.param, k, dk);
+            double sc = q;
+            if (t.sl) sc *= t.sl[i];
+            if (t.sr) sc *= t.sr[i];
+            acc[ti][0] = fma(sc, k, acc[ti][0]);
+            acc[ti][1] = fma(sc * t.coeff, dk, acc[ti][1]);
+        }
+    }
+    __shared__ double red[8][MAX_TERMS][2];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (int ti = 0; ti < b.nterms; ti++)
+        for (int h = 0; h < 2; h++) {
+            double v = acc[ti][h];
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+            if (lane == 0) red[warp][ti][h] = v;
+        }
+    __syncthreads();
+    if (threadIdx.x < 2 * b.nterms) {
+        const int ti = threadIdx.x >> 1, h = threadIdx.x & 1;
+        double v = 0.0;
+        for (int wdx = 0; wdx < 8; wdx++) v += red[wdx][ti][h];
+        atomicAdd(&g[2 * b.tix[ti] + h], v);
     }
 }
 
@@ -355,7 +422,21 @@ void launch_grad_reduce(const BlockDev& b, const double* alpha, const double* Ki
                         double* g, cudaStream_t s) {
     if (b.nrows == 0 || b.ncols == 0 || b.nterms == 0) return;
     dim3 grid((unsigned)((b.nrows + 63) / 64), (unsigned)((b.ncols + 31) / 32));
-    grad_reduce_kernel<<<grid, 256, 0, s>>>(b, alpha, Kinv, ld, w, g);
+    grad_reduce_kernel<<<grid, 256, 0, s>>>(b, LogpdfWeight{alpha, Kinv, ld}, w, g);
+    g_launch_count++;
+}
+
+void launch_grad_reduce_outer(const BlockDev& b, double a, const double* u, const double* v, double bw,
+                              const double* G, int64_t ld, double w, double* g, cudaStream_t s) {
+    if (b.nrows == 0 || b.ncols == 0 || b.nterms == 0) return;
+    dim3 grid((unsigned)((b.nrows + 63) / 64), (unsigned)((b.ncols + 31) / 32));
+    grad_reduce_kernel<<<grid, 256, 0, s>>>(b, OuterPlusDense{a, u, v, bw, G, ld}, w, g);
+    g_launch_count++;
+}
+
+void launch_grad_diag(const BlockDev& b, const double* wdiag, double* g, cudaStream_t s) {
+    if (b.nrows == 0 || b.nterms == 0) return;
+    grad_diag_kernel<<<(unsigned)((b.nrows + 255) / 256), 256, 0, s>>>(b, wdiag, g);
     g_launch_count++;
 }
 

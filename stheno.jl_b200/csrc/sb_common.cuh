@@ -105,6 +105,11 @@ void launch_assemble_diag(const BlockDev& b, double* out, cudaStream_t s);
 // off-diagonal blocks of a symmetric spec.
 void launch_grad_reduce(const BlockDev& b, const double* alpha, const double* Kinv, int64_t ld, double w,
                         double* g, cudaStream_t s);
+// the same reduction with Q_ij = a u_i v_j + bw G_ij  (sb_vfe_grad; G dense column-major, ld)
+void launch_grad_reduce_outer(const BlockDev& b, double a, const double* u, const double* v, double bw,
+                              const double* G, int64_t ld, double w, double* g, cudaStream_t s);
+// diag spec: the same two sums over the paired points i of each block, weighted by wdiag[row0 + i]
+void launch_grad_diag(const BlockDev& b, const double* wdiag, double* g, cudaStream_t s);
 
 // potrf of diagonal block k (in place in the packed matrix) + explicit inverse of L_kk
 // (dense NB x NB, ld NB) + per-block sum of log pivots + first failing pivot (1-based, 0 = ok)
@@ -168,6 +173,18 @@ void launch_transpose(const double* in, int64_t ld_in, int64_t rows, int64_t col
 void launch_pack_lower(Packed L, const double* D, int64_t ld, double shift, cudaStream_t st);
 void launch_add_diag(Packed L, const double* d, int64_t n, cudaStream_t st);
 void launch_add_dense_lower(Packed L, const double* D, int64_t ld, int64_t n, cudaStream_t st);
+// VFE gradient helpers (sb_vfe_grad)
+// D (n x n, ld n) <- s I
+void launch_set_scaled_identity(double* D, int64_t n, double s, cudaStream_t st);
+// beta[r] = (delta[r] - t[r]) / sigma2[r] for r < rows, 0 for rows <= r < rows_p
+void launch_vfe_beta(const double* delta, const double* t, const double* sigma2, int64_t rows, int64_t rows_p,
+                     double* beta, cudaStream_t st);
+// d elbo / d sigma2_r = (beta_r^2 - (1 - lb_r) / sigma2_r) / 2 + (kff_r - sigma2_r la_r) / (2 sigma2_r^2),
+// la_r = |a_r|^2, lb_r = |L_B^{-1} a_r|^2
+void launch_vfe_noise_grad(const double* beta, const double* la, const double* lb, const double* kff,
+                           const double* sigma2, int64_t rows, double* out, cudaStream_t st);
+// out[i] = -(alpha_i^2 + P[i, i]) / 2 for i < n  (d elbo / d (K_uu + jitter)_ii)
+void launch_vfe_uu_diag(const double* alpha, const double* P, int64_t ld, int64_t n, double* out, cudaStream_t st);
 
 // ---- K3': trailing update on the int8 tensor cores (wgmma, int8 Ozaki slicing), ozaki.cu ------------------
 struct alignas(64) OzMaps { unsigned char a[128]; unsigned char b[128]; };  // CUtensorMap blobs: A box (128 rows), B box (64 rows)

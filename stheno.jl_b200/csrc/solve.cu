@@ -399,7 +399,60 @@ __global__ void add_diag_kernel(Packed L, const double* __restrict__ d, int64_t 
     if (i < n) *L.at(i, i) += d[i];
 }
 
+__global__ void set_scaled_identity_kernel(double* D, int64_t n, double s) {
+    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) D[i * n + i] = s;
+}
+
+__global__ void vfe_beta_kernel(const double* __restrict__ delta, const double* __restrict__ t,
+                                const double* __restrict__ sigma2, int64_t rows, int64_t rows_p,
+                                double* __restrict__ beta) {
+    int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r < rows_p) beta[r] = r < rows ? (delta[r] - t[r]) / sigma2[r] : 0.0;
+}
+
+__global__ void vfe_noise_grad_kernel(const double* __restrict__ beta, const double* __restrict__ la,
+                                      const double* __restrict__ lb, const double* __restrict__ kff,
+                                      const double* __restrict__ sigma2, int64_t rows, double* __restrict__ out) {
+    int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= rows) return;
+    const double s = sigma2[r];
+    out[r] = 0.5 * (beta[r] * beta[r] - (1.0 - lb[r]) / s) + 0.5 * (kff[r] - s * la[r]) / (s * s);
+}
+
+__global__ void vfe_uu_diag_kernel(const double* __restrict__ alpha, const double* __restrict__ P, int64_t ld,
+                                   int64_t n, double* __restrict__ out) {
+    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) out[i] = -0.5 * (alpha[i] * alpha[i] + P[i * ld + i]);
+}
+
 }  // namespace
+
+void launch_set_scaled_identity(double* D, int64_t n, double s, cudaStream_t st) {
+    if (n <= 0) return;
+    set_scaled_identity_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(D, n, s);
+    g_launch_count++;
+}
+
+void launch_vfe_beta(const double* delta, const double* t, const double* sigma2, int64_t rows, int64_t rows_p,
+                     double* beta, cudaStream_t st) {
+    if (rows_p <= 0) return;
+    vfe_beta_kernel<<<(unsigned)((rows_p + 255) / 256), 256, 0, st>>>(delta, t, sigma2, rows, rows_p, beta);
+    g_launch_count++;
+}
+
+void launch_vfe_noise_grad(const double* beta, const double* la, const double* lb, const double* kff,
+                           const double* sigma2, int64_t rows, double* out, cudaStream_t st) {
+    if (rows <= 0) return;
+    vfe_noise_grad_kernel<<<(unsigned)((rows + 255) / 256), 256, 0, st>>>(beta, la, lb, kff, sigma2, rows, out);
+    g_launch_count++;
+}
+
+void launch_vfe_uu_diag(const double* alpha, const double* P, int64_t ld, int64_t n, double* out, cudaStream_t st) {
+    if (n <= 0) return;
+    vfe_uu_diag_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(alpha, P, ld, n, out);
+    g_launch_count++;
+}
 
 
 // whole forward (backward = true: transposed) sweep b <- L^{-1} b / L^{-T} b in ONE launch;

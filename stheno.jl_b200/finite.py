@@ -192,13 +192,19 @@ def grad_logpdf(fx: "FiniteGP", y) -> LogpdfGradient:
     fac = post.fac
     _lib.check(_lib.load().sb_logpdf_grad(fac.ctx.h, fac.h, C.byref(spec), g.ctypes.data, qd.ctypes.data))
     agg = {}
+    _aggregate_terms(agg, spec, g)
+    noise = float(qd.sum()) if np.ndim(fx.noise) == 0 else qd
+    return LogpdfGradient(noise, list(agg.values()))
+
+
+def _aggregate_terms(agg, spec, g):
+    """Add the per-term gradient g (g[2t] = d/d coeff_t, g[2t+1] = d/d log input scale_t) of `spec` into the
+    per-(leaf, kernel component) entries of `agg`."""
     for t, (atom, key, ci, kid, pair_coeff, kc, iscale) in enumerate(spec._meta):
         e = agg.setdefault((id(atom), key, ci), dict(atom=atom, component=ci, kernel_id=kid, coeff=kc,
                                                     input_scale=iscale, dcoeff=0.0, dlogscale=0.0))
         e["dcoeff"] += g[2 * t] * pair_coeff       # term coefficient = pair_coeff * kc
         e["dlogscale"] += g[2 * t + 1]
-    noise = float(qd.sum()) if np.ndim(fx.noise) == 0 else qd
-    return LogpdfGradient(noise, list(agg.values()))
 
 
 def save_factor(fx: "FiniteGP") -> np.ndarray:
@@ -483,27 +489,35 @@ class _VfeHandle:
             pass
 
 
-def _vfe_create(v: VFE, fx: FiniteGP, y):
-    fz = v.fz
-    if fz.prior is not fx.prior:
-        raise ValueError("VFE: inducing and observed FiniteGPs must share the prior")
-    if np.ndim(fx.noise) > 1:
-        raise NotImplementedError("VFE needs diagonal observation noise")
-    y = np.asarray(y, dtype=np.float64)
-    if y.shape != (len(fx),):
-        raise ValueError("DimensionMismatch: length(y) != length(fx)")
-    lz, lx = fz.lowered, fx.lowered
-    uu = spec_symmetric(lz)
-    xu = spec_dense(lx, lz)
-    ffd = spec_diag(lx)
-    nu, nf = _noise_struct(fz.noise, lz.n), _noise_struct(fx.noise, lx.n)
-    delta = np.ascontiguousarray(y - lx.mean())
+class _VfeInputs:
+    """The specs, noises and residual of elbo(VFE(fz), fx, y), built once for sb_vfe_create and sb_vfe_grad."""
+
+    def __init__(self, v: VFE, fx: FiniteGP, y):
+        fz = v.fz
+        if fz.prior is not fx.prior:
+            raise ValueError("VFE: inducing and observed FiniteGPs must share the prior")
+        if np.ndim(fx.noise) > 1:
+            raise NotImplementedError("VFE needs diagonal observation noise")
+        y = np.asarray(y, dtype=np.float64)
+        if y.shape != (len(fx),):
+            raise ValueError("DimensionMismatch: length(y) != length(fx)")
+        lz, lx = fz.lowered, fx.lowered
+        self.uu = spec_symmetric(lz)
+        self.xu = spec_dense(lx, lz)
+        self.ffd = spec_diag(lx)
+        self.nu, self.nf = _noise_struct(fz.noise, lz.n), _noise_struct(fx.noise, lx.n)
+        self.delta = np.ascontiguousarray(y - lx.mean())
+        self.n, self.m = lx.n, lz.n
+
+
+def _vfe_create(v: VFE, fx: FiniteGP, y, inputs: _VfeInputs | None = None):
+    a = inputs if inputs is not None else _VfeInputs(v, fx, y)
     h = C.c_void_p()
     out2 = (C.c_double * 2)()
     info = C.c_int64(0)
     ctx = _ctx()
-    st = _lib.load().sb_vfe_create(ctx.h, C.byref(uu), C.byref(nu), C.byref(xu), C.byref(ffd), C.byref(nf),
-                                   delta.ctypes.data, C.byref(h), out2, C.byref(info))
+    st = _lib.load().sb_vfe_create(ctx.h, C.byref(a.uu), C.byref(a.nu), C.byref(a.xu), C.byref(a.ffd),
+                                   C.byref(a.nf), a.delta.ctypes.data, C.byref(h), out2, C.byref(info))
     _lib.check(st, info)
     return _VfeHandle(h, ctx), out2[0], out2[1]
 
@@ -516,6 +530,43 @@ def elbo(v, fx=None, y=None):
 
 def dtc(v: VFE, fx: FiniteGP, y):
     return _vfe_create(v, fx, y)[2]
+
+
+class ElboGradient(LogpdfGradient):
+    """Gradient of elbo(VFE(fz), fx, y) w.r.t. the parameters the lowered plan exposes, with the elbo itself.
+
+    elbo:            the value from the same device pass (one handle build gives value and gradient).
+    noise:           d/d sigma^2 (scalar observation noise) or d/d diag(Sigma_y) (vector noise).
+    inducing_noise:  d/d jitter (scalar fz.noise) or d/d its diagonal (vector fz.noise).
+    kernels / for_atom(): as in LogpdfGradient, summed over cov(fz), cov(f, x, z) and var(f, x)."""
+
+    def __init__(self, elbo, noise, inducing_noise, kernels):
+        super().__init__(noise, kernels)
+        self.elbo, self.inducing_noise = elbo, inducing_noise
+
+
+def grad_elbo(v, fx=None, y=None) -> ElboGradient:
+    """d elbo(VFE(fz), fx, y) / d theta on the device (also grad_elbo(sparse::SparseFiniteGP, y)): the reverse
+    pass of sb_vfe_create streams K_fu in the same chunks (DESIGN.md §4)."""
+    if isinstance(v, SparseFiniteGP):
+        return grad_elbo(VFE(v.finducing), v.fobs, fx)
+    if np.ndim(v.fz.noise) > 1:
+        raise NotImplementedError("grad_elbo: scalar or diagonal inducing-point noise")
+    a = _VfeInputs(v, fx, y)
+    handle, e, _ = _vfe_create(v, fx, y, a)
+    g_uu = np.zeros(2 * max(1, a.uu.nterms))
+    g_xu = np.zeros(2 * max(1, a.xu.nterms))
+    g_ff = np.zeros(2 * max(1, a.ffd.nterms))
+    g_nu, g_nf = np.empty(a.m), np.empty(a.n)
+    _lib.check(_lib.load().sb_vfe_grad(
+        handle.ctx.h, handle.h, C.byref(a.uu), C.byref(a.xu), C.byref(a.ffd), C.byref(a.nf), a.delta.ctypes.data,
+        g_uu.ctypes.data, g_xu.ctypes.data, g_ff.ctypes.data, g_nu.ctypes.data, g_nf.ctypes.data))
+    agg = {}
+    for spec, g in ((a.uu, g_uu), (a.xu, g_xu), (a.ffd, g_ff)):
+        _aggregate_terms(agg, spec, g)
+    noise = float(g_nf.sum()) if np.ndim(fx.noise) == 0 else g_nf
+    inducing = float(g_nu.sum()) if np.ndim(v.fz.noise) == 0 else g_nu
+    return ElboGradient(e, noise, inducing, list(agg.values()))
 
 
 class ApproxPosteriorGP:

@@ -437,6 +437,37 @@ function logpdf_grad(fx::B200Finite, y::AbstractVector{<:Real})
     g, qd
 end
 
+# ---- gradient of the elbo (reverse mode of elbo(VFE(fz), fx, y), sparse_finite_gp.jl:52-58) ---------------
+# returns (elbo, g_uu, g_xu, g_ff, g_noise_u, g_noise_f): per term of cov(fz) / cov(f, x, z) / var(f, x) as in
+# logpdf_grad, g_noise_u[i] = d/d (K_uu + jitter)[i,i], g_noise_f[i] = d/d Sigma_y[i,i].  The specs are built
+# once and passed to both sb_vfe_create and sb_vfe_grad.
+function elbo_grad(v::AbstractGPs.VFE{<:B200Finite}, fx::B200Finite, y::AbstractVector{<:Real})
+    fz = v.fz
+    fz.f === fx.f || throw(ArgumentError("VFE: inducing and observed FiniteGPs must share the prior"))
+    length(y) == npoints(fx.x) || throw(DimensionMismatch("length(y) != length(fx)"))
+    fx.Σy isa Diagonal || error("SthenoB200: VFE needs diagonal observation noise")
+    pz, vz = components(fz.f, fz.x); px, vx = components(fx.f, fx.x)
+    uu, k1 = build_spec(pz, vz, pz, vz; which=:sym)
+    xu, k2 = build_spec(px, vx, pz, vz; which=:all)
+    ffd, k3 = build_spec(px, vx, px, vx; which=:diag)
+    nu, ndu = noise_struct(fz.Σy); nf, ndf = noise_struct(fx.Σy)
+    δ = Float64.(y .- host_mean(fx))
+    h = Ref{Ptr{Cvoid}}(C_NULL); out2 = zeros(2); info = Ref{Int64}(0)
+    st = GC.@preserve k1 k2 k3 ndu ndf δ out2 ccall((:sb_vfe_create, LIB), Int32,
+        (Ptr{Cvoid}, Ref{SbCovSpec}, Ref{SbNoise}, Ref{SbCovSpec}, Ref{SbCovSpec}, Ref{SbNoise}, Ptr{Cvoid},
+         Ref{Ptr{Cvoid}}, Ptr{Float64}, Ref{Int64}),
+        ctx().h, uu, nu, xu, ffd, nf, δ, h, out2, info)
+    check(st, info[])
+    V = VfeHandle(h[]); finalizer(destroy!, V)
+    guu = zeros(2 * max(1, Int(uu.nterms))); gxu = zeros(2 * max(1, Int(xu.nterms)))
+    gff = zeros(2 * max(1, Int(ffd.nterms))); gnu = zeros(npoints(fz.x)); gnf = zeros(npoints(fx.x))
+    GC.@preserve k1 k2 k3 ndf δ guu gxu gff gnu gnf check(ccall((:sb_vfe_grad, LIB), Int32,
+        (Ptr{Cvoid}, Ptr{Cvoid}, Ref{SbCovSpec}, Ref{SbCovSpec}, Ref{SbCovSpec}, Ref{SbNoise}, Ptr{Cvoid},
+         Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Cvoid}, Ptr{Cvoid}),
+        ctx().h, V.h, uu, xu, ffd, nf, δ, guu, gxu, gff, gnu, gnf))
+    out2[1], guu, gxu, gff, gnu, gnf
+end
+
 # ---- factor checkpoint / resume --------------------------------------------------------------------------
 function save_factor(F::Factor)
     n = Ref{Int64}(0)
@@ -469,6 +500,6 @@ end
 set_option!(key::AbstractString, value::Integer) =
     check(ccall((:sb_ctx_set_option, LIB), Int32, (Ptr{Cvoid}, Cstring, Int64), ctx().h, key, value))
 
-export b200, B200GPPP, timings, set_option!, logpdf_grad, save_factor, load_factor
+export b200, B200GPPP, timings, set_option!, logpdf_grad, elbo_grad, save_factor, load_factor
 
 end # module

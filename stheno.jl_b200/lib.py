@@ -58,7 +58,7 @@ EXPORTS = [
     "sb_factor_destroy", "sb_factor_logdet", "sb_logpdf", "sb_factor_set_data", "sb_factor_alpha",
     "sb_factor_set_alpha", "sb_predict", "sb_predict_cov", "sb_predict_factor", "sb_rand", "sb_factor_get_L",
     "sb_vfe_create", "sb_vfe_predict", "sb_vfe_predict_cov", "sb_vfe_destroy",
-    "sb_factor_export_size", "sb_factor_export", "sb_factor_import", "sb_logpdf_grad",
+    "sb_factor_export_size", "sb_factor_export", "sb_factor_import", "sb_logpdf_grad", "sb_vfe_grad",
 ]
 
 _lib = None
@@ -121,6 +121,8 @@ def load():
         "sb_factor_import": [vp, vp, i64, P(vp)],
         "sb_vfe_create": [vp, P(sb_covspec), P(sb_noise), P(sb_covspec), P(sb_covspec), P(sb_noise), vp,
                           P(vp), P(C.c_double), P(i64)],
+        "sb_vfe_grad": [vp, vp, P(sb_covspec), P(sb_covspec), P(sb_covspec), P(sb_noise), vp,
+                        vp, vp, vp, vp, vp],
         "sb_vfe_predict": [vp, vp, P(sb_covspec), P(sb_covspec), vp, vp],
         "sb_vfe_predict_cov": [vp, vp, P(sb_covspec), P(sb_covspec), vp],
         "sb_vfe_destroy": [vp],
