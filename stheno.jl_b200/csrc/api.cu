@@ -683,71 +683,53 @@ constexpr int SWEEP_COLS = OUTER_BLOCKS * NB;  // columns of the Xk workspace (r
 
 // W <- W L^{-T} (rows_p x Np, ld rows_p): right-looking block forward substitution, tensor-core
 // products only.  keep: write the result back into W; acc != null: acc[r] += sum_c result[r,c]^2.
-// Xk: rows_p x 512 workspace.  With a int8-Ozaki factor (f->oz) the big update of each outer
-// step (4 block columns, K = 512) runs on the int8 Ozaki kernel; the small in-step products stay DMMA.
+// Xk: rows_p x 512 workspace.  Each outer step solves 4 block columns (small in-step DMMA products)
+// and then applies them to the rest of W in one big update with K = 512, which reads and writes the
+// remaining columns of W once per 4 block columns.  That update runs on DMMA, or on the int8 Ozaki
+// kernel for an int8-Ozaki factor (f->oz) given its workspace.
 static int32_t trsm_sweep(sb_ctx* c, sb_factor* f, double* W, int64_t rows_p, double* Xk, bool keep, double* acc,
                           OzSweepWs* ws = nullptr) {
     const int64_t nblk = f->L.nblk(), Np = f->Np;
-    if (f->oz && ws && ws->ready) {
-        for (int64_t k0 = 0; k0 < nblk; k0 += OUTER_BLOCKS) {
-            const int nq = outer_width(nblk, k0);
-            double* X[OUTER_BLOCKS];
-            for (int q = 0; q < nq; q++) {
-                const int64_t kq = k0 + q;
-                double* Wq = W + kq * NB * rows_p;
-                X[q] = Xk + (int64_t)q * NB * rows_p;
-                if (q > 0) {  // bring block column kq up to date with the X panels of this outer step
-                    const double* As[OUTER_BLOCKS]; int64_t las[OUTER_BLOCKS];
-                    const double* Bs[OUTER_BLOCKS]; int64_t lbs[OUTER_BLOCKS];
-                    for (int p = 0; p < q; p++) { As[p] = X[p]; las[p] = rows_p; Bs[p] = f->L.blk(kq, k0 + p); lbs[p] = f->L.ld(k0 + p); }
-                    launch_gemm_nt_seg(q, As, las, Bs, lbs, Wq, rows_p, rows_p, NB, -1.0, 1.0, c->stream);
-                }
-                launch_gemm_nt(Wq, rows_p, f->invL + kq * (int64_t)NB * NB, NB, X[q], rows_p, rows_p, NB, NB, 1.0, 0.0, c->stream);
-                if (keep) SB_CUDA(cudaMemcpyAsync(Wq, X[q], (size_t)rows_p * NB * sizeof(double), cudaMemcpyDeviceToDevice, c->stream));
-                if (acc) launch_rowsumsq_acc(X[q], rows_p, rows_p, NB, acc, c->stream);
+    const bool oz = f->oz && ws && ws->ready;
+    const int64_t las[OUTER_BLOCKS] = {rows_p, rows_p, rows_p, rows_p};
+    for (int64_t k0 = 0; k0 < nblk; k0 += OUTER_BLOCKS) {
+        const int nq = outer_width(nblk, k0);
+        const double* X[OUTER_BLOCKS];
+        for (int q = 0; q < nq; q++) {
+            const int64_t kq = k0 + q;
+            double* Wq = W + kq * NB * rows_p;
+            double* Xq = Xk + (int64_t)q * NB * rows_p;
+            X[q] = Xq;
+            if (q > 0) {  // bring block column kq up to date with the X panels of this outer step
+                const double* Bs[OUTER_BLOCKS]; int64_t lbs[OUTER_BLOCKS];
+                for (int p = 0; p < q; p++) { Bs[p] = f->L.blk(kq, k0 + p); lbs[p] = f->L.ld(k0 + p); }
+                launch_gemm_nt_seg(q, X, las, Bs, lbs, Wq, rows_p, rows_p, NB, -1.0, 1.0, c->stream);
             }
-            const int64_t jt = k0 + nq, m = Np - jt * NB;
-            if (m <= 0) break;
-            OzSrc sx{}, sl{};
-            sx.nseg = sl.nseg = nq;
-            for (int q = 0; q < nq; q++) {
-                sx.base[q] = X[q]; sx.ld[q] = rows_p; sx.rbs[q] = NB;
-                sl.base[q] = f->L.blk(jt, k0 + q); sl.ld[q] = f->L.ld(k0 + q); sl.rbs[q] = NB;
-            }
-            launch_oz_slice(sx, 0, rows_p / NB, 0, ws->rows, ws->scale.d(), reinterpret_cast<int*>(ws->expo.p),
-                            reinterpret_cast<signed char*>(ws->planes.p), c->stream);
-            launch_oz_slice(sl, 0, m / NB, jt * (int64_t)NB, Np, f->oz_scale[0], f->oz_expo[0], f->oz_planes[0], c->stream);
-            if (launch_gemm_ozaki(W + jt * NB * rows_p, rows_p, rows_p, m, nq, &ws->maps, ws->scale.d(), 0, &f->oz_maps[0],
-                                  f->oz_scale[0], jt * (int64_t)NB, c->stream) != 0) {
-                sb::set_error("int8 Ozaki sweep kernel could not be launched");
-                return SB_ERR_CUDA;
-            }
+            launch_gemm_nt(Wq, rows_p, f->invL + kq * (int64_t)NB * NB, NB, Xq, rows_p, rows_p, NB, NB, 1.0, 0.0, c->stream);
+            if (keep) SB_CUDA(cudaMemcpyAsync(Wq, Xq, (size_t)rows_p * NB * sizeof(double), cudaMemcpyDeviceToDevice, c->stream));
+            if (acc) launch_rowsumsq_acc(Xq, rows_p, rows_p, NB, acc, c->stream);
         }
-        SB_CUDA(cudaGetLastError());
-        return SB_OK;
-    }
-    // DMMA path: two block columns per outer step so the big update runs at K = 256
-    double* X0 = Xk;
-    double* X1 = Xk + rows_p * NB;
-    for (int64_t k0 = 0; k0 < nblk; k0 += 2) {
-        const int64_t k1 = k0 + 1;
-        double* W0 = W + k0 * NB * rows_p;
-        launch_gemm_nt(W0, rows_p, f->invL + k0 * (int64_t)NB * NB, NB, X0, rows_p, rows_p, NB, NB, 1.0, 0.0, c->stream);
-        if (keep) SB_CUDA(cudaMemcpyAsync(W0, X0, (size_t)rows_p * NB * sizeof(double), cudaMemcpyDeviceToDevice, c->stream));
-        if (acc) launch_rowsumsq_acc(X0, rows_p, rows_p, NB, acc, c->stream);
-        if (k1 >= nblk) break;
-        double* W1 = W + k1 * NB * rows_p;
-        launch_gemm_nt(X0, rows_p, f->L.blk(k1, k0), f->L.ld(k0), W1, rows_p, rows_p, NB, NB, -1.0, 1.0, c->stream);
-        launch_gemm_nt(W1, rows_p, f->invL + k1 * (int64_t)NB * NB, NB, X1, rows_p, rows_p, NB, NB, 1.0, 0.0, c->stream);
-        if (keep) SB_CUDA(cudaMemcpyAsync(W1, X1, (size_t)rows_p * NB * sizeof(double), cudaMemcpyDeviceToDevice, c->stream));
-        if (acc) launch_rowsumsq_acc(X1, rows_p, rows_p, NB, acc, c->stream);
-        const int64_t m = Np - (k1 + 1) * NB;
-        if (m > 0) {
-            const double* As[2] = {X0, X1};
-            const int64_t las[2] = {rows_p, rows_p};
-            const double* Bs[2] = {f->L.blk(k1 + 1, k0), f->L.blk(k1 + 1, k1)};
-            const int64_t lbs[2] = {f->L.ld(k0), f->L.ld(k1)};
-            launch_gemm_nt_seg(2, As, las, Bs, lbs, W + (k1 + 1) * NB * rows_p, rows_p, rows_p, m, -1.0, 1.0, c->stream);
+        const int64_t jt = k0 + nq, m = Np - jt * NB;
+        if (m <= 0) break;
+        if (!oz) {  // W[:, jt..] -= [X_0 .. X_nq-1] [L(jt.., k0) .. L(jt.., k0+nq-1)]^T
+            const double* Ls[OUTER_BLOCKS]; int64_t lls[OUTER_BLOCKS];
+            for (int q = 0; q < nq; q++) { Ls[q] = f->L.blk(jt, k0 + q); lls[q] = f->L.ld(k0 + q); }
+            launch_gemm_nt_seg(nq, X, las, Ls, lls, W + jt * NB * rows_p, rows_p, rows_p, m, -1.0, 1.0, c->stream);
+            continue;
+        }
+        OzSrc sx{}, sl{};
+        sx.nseg = sl.nseg = nq;
+        for (int q = 0; q < nq; q++) {
+            sx.base[q] = X[q]; sx.ld[q] = rows_p; sx.rbs[q] = NB;
+            sl.base[q] = f->L.blk(jt, k0 + q); sl.ld[q] = f->L.ld(k0 + q); sl.rbs[q] = NB;
+        }
+        launch_oz_slice(sx, 0, rows_p / NB, 0, ws->rows, ws->scale.d(), reinterpret_cast<int*>(ws->expo.p),
+                        reinterpret_cast<signed char*>(ws->planes.p), c->stream);
+        launch_oz_slice(sl, 0, m / NB, jt * (int64_t)NB, Np, f->oz_scale[0], f->oz_expo[0], f->oz_planes[0], c->stream);
+        if (launch_gemm_ozaki(W + jt * NB * rows_p, rows_p, rows_p, m, nq, &ws->maps, ws->scale.d(), 0, &f->oz_maps[0],
+                              f->oz_scale[0], jt * (int64_t)NB, c->stream) != 0) {
+            sb::set_error("int8 Ozaki sweep kernel could not be launched");
+            return SB_ERR_CUDA;
         }
     }
     SB_CUDA(cudaGetLastError());

@@ -30,9 +30,10 @@ constexpr int LOOKAHEAD_SMS = 8;
 // the panel chain, not the trailing update, can set the pace of the second half of the factorisation.
 // Pick the reservation that balances  T^B * S/(S-r)  against  serial chain + panel GEMM work / r.
 // Per-tile cost: time per SM of one 128 x 64 half-tile with K = 512 (2*128*64*512 flop) at the DMMA
-// trailing-update rate bench.py measured at N = 65536 on one H100 80GB (700 W), 28.1 TFLOP/s over 132 SMs.
-// The serial-chain latencies below have not been measured on H100.
-constexpr double DMMA_HALF_TILE_US = 39.5;
+// trailing-update rate bench.py measured at N = 65536 on one H100 80GB (700 W), 29.2 TFLOP/s over 132 SMs.
+// It sizes the multi-GPU look-ahead reservation only.  The serial-chain latencies below have not been
+// measured on H100.
+constexpr double DMMA_HALF_TILE_US = 37.9;
 static int pick_lookahead_sms(int num_sms, double tilesB_half, int nq_next, int64_t rows_next) {
     const double serial_us = nq_next * 230.0;   // potrf + exchange latency; unmeasured
     // DMMA half-tiles of the next panel phase: TRSM (nq panels) + catch-up (0 + 1 + 2 + 3 segments)

@@ -7,13 +7,18 @@
 // the `C.U' \ K_fx` solves of AbstractGPs (SURVEY.md App. A).
 //
 // sm_90a notes.  wgmma has no fp64 kind, so fp64 tensor math is the DMMA path
-// (mma.sync.m8n8k4.f64 -> SASS DMMA.8x8x4).  Operand k-slabs are staged global->shared by the
+// (mma.sync.m16n8k4.f64 -> SASS DMMA.16x8x4).  Operand k-slabs are staged global->shared by the
 // TMA engine with 1-D bulk copies (cp.async.bulk ... mbarrier::complete_tx -> SASS UBLKCP) into a
 // 4-stage ring; one mbarrier per stage.  Shared tiles are [k][row] with a 4-double pad so the
-// m8n8k4 fragment loads (8 rows x 4 k per operand) are bank-conflict free.  The MMA is issued
+// fragment loads (8 rows x 4 k per LDS.64) are bank-conflict free.  The MMA is issued
 // "transposed" (m <-> C columns, n <-> C rows) so each thread owns 2 consecutive rows of C and
 // the epilogue uses 16-byte loads/stores.  CTA tile 128x64, 8 warps of 32x32, 2 CTAs per SM so
-// one CTA's C read-modify-write epilogue overlaps the other's MMA main loop.
+// one CTA's C read-modify-write epilogue overlaps the other's MMA main loop.  Two CTAs of 9 warps
+// cap the kernel at 96 registers: each of the SM's 4 sub-partitions holds 16384 registers and
+// some sub-partition gets 5 of the 18 warps (5 * 32 * 96 <= 16384 < 5 * 32 * 104).  At 112 registers
+// only one CTA fits and the kernel is slower.  On H100 DMMA.8x8x4 (m8n8k4) issues at half the fp64
+// tensor rate of the m16n8k{4,8,16} shapes (profiles/mb_dmma_loop_h100.txt); m16n8k4 is the one
+// whose fragments fit the 96-register budget.
 #include "sb_common.cuh"
 
 namespace sb {
@@ -89,11 +94,13 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
         ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar))
         : "memory");
 }
-__device__ __forceinline__ void dmma(double (&c)[2], double a, double b) {
+// c[0..1] = C(m = gid, n = 2 tig + 0..1), c[2..3] = C(m = gid + 8, ...);
+// a0 = A(m = gid, k = tig), a1 = A(m = gid + 8, k = tig), b = B(k = tig, n = gid)
+__device__ __forceinline__ void dmma(double (&c)[4], double a0, double a1, double b) {
     asm volatile(
-        "mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
-        : "+d"(c[0]), "+d"(c[1])
-        : "d"(a), "d"(b));
+        "mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
+        : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
+        : "d"(a0), "d"(a1), "d"(b));
 }
 
 // TILED layout of a panel (written by the TRSM epilogue, read by the SYRK): for every 128-row
@@ -252,20 +259,19 @@ __global__ void __launch_bounds__(THREADS, 2) gemm_nt_kernel(const __grid_consta
     const int wr = warp & 3, wc = warp >> 2;  // 4 warps along rows, 2 along cols; 32x32 each
     const double alpha = g.alpha, beta = g.beta;
     const double* a_base = sA + wr * 32 + gid + tig * LDA_S;
-    const double* b_base0 = sB + wc * 32 + gid + tig * LDB_S;
+    const double* b_base = sB + wc * 32 + gid + tig * LDB_S;
     int slot = 0;
     uint32_t phase = 0;
     TileCursor cur;
     cur.init(g, blockIdx.x);
     for (; cur.t < g.total_tiles; cur.advance(g, gridDim.x)) {
-        double acc[4][4][2];
+        // acc[jj][i][2h + e] = C(column wc*32 + (2jj + h)*8 + gid, row wr*32 + i*8 + 2tig + e)
+        double acc[2][4][4];
 #pragma unroll
-        for (int j = 0; j < 4; j++)
+        for (int jj = 0; jj < 2; jj++)
 #pragma unroll
-            for (int i = 0; i < 4; i++) acc[j][i][0] = acc[j][i][1] = 0.0;
+            for (int i = 0; i < 4; i++) acc[jj][i][0] = acc[jj][i][1] = acc[jj][i][2] = acc[jj][i][3] = 0.0;
 
-        const TilePtrs tp = cur.ptrs(g);
-        const double* b_base = b_base0;
         for (int c = 0; c < nchunks; c++) {
 #ifndef SB_ABLATE_NO_TMA
             mbar_wait(&full[slot], phase);
@@ -280,9 +286,9 @@ __global__ void __launch_bounds__(THREADS, 2) gemm_nt_kernel(const __grid_consta
 #pragma unroll
                 for (int j = 0; j < 4; j++) cf[j] = b[k4 * 4 * LDB_S + j * 8];
 #pragma unroll
-                for (int j = 0; j < 4; j++)
+                for (int jj = 0; jj < 2; jj++)
 #pragma unroll
-                    for (int i = 0; i < 4; i++) dmma(acc[j][i], cf[j], rf[i]);
+                    for (int i = 0; i < 4; i++) dmma(acc[jj][i], cf[2 * jj], cf[2 * jj + 1], rf[i]);
             }
             __syncwarp();
 #ifndef SB_ABLATE_NO_TMA
@@ -291,7 +297,9 @@ __global__ void __launch_bounds__(THREADS, 2) gemm_nt_kernel(const __grid_consta
             if (++slot == STAGES) { slot = 0; phase ^= 1; }
         }
 
-        // epilogue: thread owns rows (2*tig, 2*tig+1) of column gid in each 8x8 fragment
+        // (the tile's C pointers are formed only now: held across the main loop they cost registers)
+        const TilePtrs tp = cur.ptrs(g);
+        // epilogue: thread owns rows (2*tig, 2*tig+1) of column gid in each 8x8 quarter of a fragment
         // tiled output (TRSM -> panel in slab-image layout): column k of row tile rt is the padded
         // 132-double column ((rt*128 + k) * 132); this tile covers k = ct*64 .. ct*64+63
         double* cbase = g.c_tiled
@@ -314,8 +322,8 @@ __global__ void __launch_bounds__(THREADS, 2) gemm_nt_kernel(const __grid_consta
                     for (int i = 0; i < 4; i++) {
                         const int j = jh * 2 + jj;
                         double2 o;
-                        o.x = fma(alpha, acc[j][i][0], beta * old[jj][i].x);
-                        o.y = fma(alpha, acc[j][i][1], beta * old[jj][i].y);
+                        o.x = fma(alpha, acc[jh][i][2 * jj], beta * old[jj][i].x);
+                        o.y = fma(alpha, acc[jh][i][2 * jj + 1], beta * old[jj][i].y);
                         *reinterpret_cast<double2*>(cbase + (int64_t)j * 8 * ldc + i * 8) = o;
                     }
             }
@@ -324,7 +332,7 @@ __global__ void __launch_bounds__(THREADS, 2) gemm_nt_kernel(const __grid_consta
             for (int j = 0; j < 4; j++)
 #pragma unroll
                 for (int i = 0; i < 4; i++) {
-                    double2 o = make_double2(alpha * acc[j][i][0], alpha * acc[j][i][1]);
+                    double2 o = make_double2(alpha * acc[j >> 1][i][2 * (j & 1)], alpha * acc[j >> 1][i][2 * (j & 1) + 1]);
                     *reinterpret_cast<double2*>(cbase + (int64_t)j * 8 * ldc + i * 8) = o;
                 }
         }

@@ -12,6 +12,13 @@ int main(int argc, char** argv) {
     double *A, *B, *C;
     CK(cudaMalloc(&A, M * KMAX * 8)); CK(cudaMalloc(&B, N * KMAX * 8)); CK(cudaMalloc(&C, M * N * 8));
     CK(cudaMemset(A, 0, M * KMAX * 8)); CK(cudaMemset(B, 0, N * KMAX * 8)); CK(cudaMemset(C, 0, M * N * 8));
+    {   // the kernel is built around 2 CTAs per SM (one CTA's epilogue overlaps the other's main loop)
+        CK(cudaFuncSetAttribute(sb::gemm_nt_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sb::SMEM_BYTES));
+        cudaFuncAttributes fa; CK(cudaFuncGetAttributes(&fa, sb::gemm_nt_kernel));
+        int fit = 0; CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&fit, sb::gemm_nt_kernel, sb::THREADS, sb::SMEM_BYTES));
+        printf("{\"kernel\":\"gemm_nt_kernel\",\"regs\":%d,\"local_bytes\":%zu,\"smem_bytes\":%zu,\"ctas_per_sm\":%d}\n",
+               fa.numRegs, fa.localSizeBytes, sb::SMEM_BYTES, fit);
+    }
     cudaEvent_t e0, e1; CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
     for (double beta : {1.0, 0.0})
         for (int64_t K : {128, 256, 512, 1024, 4096}) {
