@@ -216,6 +216,16 @@ int32_t sb_rand(sb_ctx* ctx, sb_factor* f, const void* z, int32_t S, void* out);
  * factorised on the device; the returned handle works with sb_rand / sb_logpdf / sb_factor_logdet. */
 int32_t sb_predict_factor(sb_ctx* ctx, sb_factor* f, const sb_covspec* cross, const sb_covspec* prior_full,
                           const sb_noise* noise, sb_factor** out, int64_t* info);
+/* sb_factor_append replaces posterior(f_post(x2, Sigma2), y2)'s factor update (AbstractGPs update_chol):
+ * *out = cholesky of the covariance of the stacked observations [x; x2] with block-diagonal noise
+ * (f's own noise, then Sigma2).  cross = cov(prior, x2, x) dense spec (N2 x N, all blocks); prior_full =
+ * cov(prior, x2) dense spec (N2 x N2) -- the same two specs sb_predict_factor takes.  f is not modified;
+ * the new handle has no alpha (call sb_factor_set_data).  On SB_ERR_NOT_POSDEF *info is the 1-based
+ * pivot in the JOINT order (> N).  Multi-GPU: every rank calls it; the work is replicated (no communication).
+ * Cost O(N2 N^2 + N2^2 N + N2^3): f's full 128-wide block columns are kept, only the rows of its partial
+ * last block are factorised again together with the new ones. */
+int32_t sb_factor_append(sb_ctx* ctx, sb_factor* f, const sb_covspec* cross, const sb_covspec* prior_full,
+                         const sb_noise* noise, sb_factor** out, int64_t* info);
 /* sb_logpdf_grad replaces the reverse-mode pass through logpdf(fx, y) (Zygote + the ChainRules
  * glue of src/affine_transformations/cross.jl:8-22; examples/getting_started/script.jl:154-213):
  *   dlogpdf/dtheta = 1/2 tr((alpha alpha' - K^{-1}) dK/dtheta)

@@ -736,11 +736,40 @@ static int32_t trsm_sweep(sb_ctx* c, sb_factor* f, double* W, int64_t rows_p, do
     return SB_OK;
 }
 
-// shared body of sb_predict / sb_predict_cov
+// Joint factor of the observations [old; new] (sb_factor_append).  h = NB floor(N1 / NB) is the head (f's full
+// block columns), r = N1 - h.  Block columns j < h / NB: f's rows [NB j, N1), then the N2 rows of V = K21 L^{-T}
+// (V: rows_p x Np1, ld ldv, from the sweep).  The rest: S, the factor of the Schur complement of the head,
+// order r + N2, whose packed storage is the tail of the joint one (both start on the block boundary h).
+static int32_t factor_splice(sb_ctx* c, const sb_factor* f, const sb_factor* S, const double* V, int64_t ldv,
+                             int64_t N2, std::unique_ptr<sb_factor>& out) {
+    const int64_t nh = f->N / NB, h = nh * NB;
+    std::unique_ptr<sb_factor> g;
+    SB_TRY(factor_alloc(c, h + S->N, g));
+    SB_CHECK(g->Np - h == S->Np, "append: Schur factor does not match the joint layout");
+    const int64_t nblk = g->L.nblk();
+    launch_append_relayout(g->L, f->L, f->N, N2, V, ldv, h, c->stream);
+    SB_CUDA(cudaMemcpyAsync(g->L.base + g->L.off(nh), S->L.base, (size_t)S->L.total() * sizeof(double),
+                            cudaMemcpyDeviceToDevice, c->stream));
+    SB_CUDA(cudaMemcpyAsync(g->invL, f->invL, (size_t)h * NB * sizeof(double), cudaMemcpyDeviceToDevice, c->stream));
+    SB_CUDA(cudaMemcpyAsync(g->invL + h * NB, S->invL, S->invL.bytes, cudaMemcpyDeviceToDevice, c->stream));
+    SB_CUDA(cudaMemcpyAsync(g->logdet_blk, f->logdet_blk, nh * sizeof(double), cudaMemcpyDeviceToDevice, c->stream));
+    SB_CUDA(cudaMemcpyAsync(g->logdet_blk + nh, S->logdet_blk, S->logdet_blk.bytes, cudaMemcpyDeviceToDevice, c->stream));
+    SB_CUDA(cudaGetLastError());
+    std::vector<double> ld(nblk);
+    SB_CUDA(cudaMemcpyAsync(ld.data(), g->logdet_blk, nblk * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    SB_CUDA(cudaStreamSynchronize(c->stream));
+    double sum = 0.0;   // summed in block order, as factor_finish does for a fresh factor
+    for (double v : ld) sum += v;
+    g->logdet = sum;
+    out = std::move(g);
+    return SB_OK;
+}
+
+// shared body of sb_predict / sb_predict_cov / sb_predict_factor / sb_factor_append
 static int32_t predict_impl(sb_ctx* c, sb_factor* f, const sb_covspec* cross,
                             const sb_covspec* prior, bool full_cov, void* mean_out, void* var_out,
                             void* cov_out, const sb_noise* post_noise = nullptr, sb_factor** fac_out = nullptr,
-                            int64_t* info = nullptr) {
+                            int64_t* info = nullptr, bool append = false) {
     begin_call(c);
     int64_t before = g_launch_count;
     SB_CHECK(cross->ncols == f->N, "cross spec must be N* x N");
@@ -819,24 +848,40 @@ static int32_t predict_impl(sb_ctx* c, sb_factor* f, const sb_covspec* cross,
                 SB_CUDA(cudaMemcpy2DAsync(cov_out, Ns * sizeof(double), Cm.p, Nsp * sizeof(double),
                                           Ns * sizeof(double), Ns, cudaMemcpyDefault, c->stream));
             if (fac_out) {
-                // posterior covariance (+ noise) -> packed layout -> Cholesky, all on device
-                DevBuf nd(c), ndn(c);
-                std::unique_ptr<sb_factor> fn;
-                SB_TRY(factor_alloc(c, Ns, fn));
-                double s2 = post_noise ? post_noise->sigma2 : 0.0;
-                const bool pn_dense = post_noise && post_noise->dense;
-                launch_pack_lower(fn->L, Cm.d(), Nsp, (pn_dense || (post_noise && post_noise->diag)) ? 0.0 : s2, c->stream);
-                if (pn_dense) {  // f_post(x*, Sigma_dense): add the lower triangle of the full noise matrix
-                    SB_TRY(ndn.alloc((size_t)Ns * Ns * sizeof(double)));
-                    SB_CUDA(cudaMemcpyAsync(ndn.p, post_noise->dense, (size_t)Ns * Ns * sizeof(double), cudaMemcpyDefault, c->stream));
-                    launch_add_dense_lower(fn->L, ndn.d(), Ns, Ns, c->stream);
-                } else if (post_noise && post_noise->diag) {
-                    SB_TRY(nd.alloc(Ns * sizeof(double)));
-                    SB_CUDA(cudaMemcpyAsync(nd.p, post_noise->diag, Ns * sizeof(double), cudaMemcpyDefault, c->stream));
-                    launch_add_diag(fn->L, nd.d(), Ns, c->stream);
+                // posterior covariance (+ noise) -> packed layout -> Cholesky, all on device.  append: the
+                // matrix factorised is the Schur complement S of the old head (see factor_splice), whose first
+                // r rows are the old rows of f's partial last block; otherwise r = 0 and S = Cm + noise.
+                const int64_t h = append ? f->N / NB * NB : 0;
+                const int r = (int)(append ? f->N - h : 0);
+                DevBuf nd(c);
+                const bool pn_dense = post_noise && post_noise->dense, pn_diag = post_noise && post_noise->diag;
+                if (pn_dense || pn_diag) {
+                    const size_t n = pn_dense ? (size_t)Ns * Ns : (size_t)Ns;
+                    SB_TRY(nd.alloc(n * sizeof(double)));
+                    SB_CUDA(cudaMemcpyAsync(nd.p, pn_dense ? post_noise->dense : post_noise->diag, n * sizeof(double),
+                                            cudaMemcpyDefault, c->stream));
                 }
-                launch_fill_padding(fn->L, Ns, c->stream);
-                SB_TRY(factor_finish(c, fn.get(), info, /*force_local=*/true));
+                launch_add_noise_dense(Cm.d(), Nsp, Ns, post_noise ? post_noise->sigma2 : 0.0, pn_diag && !pn_dense ? nd.d() : nullptr,
+                                       pn_dense ? nd.d() : nullptr, c->stream);
+                std::unique_ptr<sb_factor> fn;
+                SB_TRY(factor_alloc(c, r + Ns, fn));
+                launch_pack_schur(fn->L, r + Ns, r, Cm.d(), Nsp, r ? f->L.blk(h / NB, h / NB) : nullptr, f->L.ld(h / NB),
+                                  r ? W.d() + h * Nsp : nullptr, Nsp, c->stream);
+                launch_fill_padding(fn->L, r + Ns, c->stream);
+                int64_t info_s = 0;
+                const int32_t st = factor_finish(c, fn.get(), &info_s, /*force_local=*/true);
+                if (st == SB_ERR_NOT_POSDEF) {   // S's pivot index, in the order of the joint matrix
+                    if (info) *info = h + info_s;
+                    if (h > 0)
+                        sb::set_error("matrix is not positive definite; Cholesky factorization failed at pivot " +
+                                      std::to_string(h + info_s));
+                }
+                SB_TRY(st);
+                if (h > 0) {
+                    std::unique_ptr<sb_factor> joint;
+                    SB_TRY(factor_splice(c, f, fn.get(), W.d(), Nsp, Ns, joint));
+                    fn = std::move(joint);
+                }
                 *fac_out = fn.release();
             }
             SB_CUDA(cudaStreamSynchronize(c->stream));
@@ -881,6 +926,18 @@ int32_t sb_predict_factor(sb_ctx* c, sb_factor* f, const sb_covspec* cross, cons
     *out = nullptr;
     if (info) *info = 0;
     return predict_impl(c, f, cross, prior_full, true, nullptr, nullptr, nullptr, noise, out, info);
+}
+
+// Sequential conditioning without refactorising (AbstractGPs update_chol): the sweep V = K21 L^{-T} and
+// P = K22 + Sigma2 - V V' are sb_predict_factor's; then only the Schur complement of f's full block columns is
+// factorised and spliced behind them (factor_splice).  O(N2 N1^2 + N2^2 N1 + N2^3) against (N1 + N2)^3 / 3.
+int32_t sb_factor_append(sb_ctx* c, sb_factor* f, const sb_covspec* cross, const sb_covspec* prior_full,
+                         const sb_noise* noise, sb_factor** out, int64_t* info) {
+    SB_CHECK(c && f && cross && prior_full && out, "null argument");
+    *out = nullptr;
+    if (info) *info = 0;
+    SB_CHECK(cross->nrows > 0, "sb_factor_append: no new observations");
+    return predict_impl(c, f, cross, prior_full, true, nullptr, nullptr, nullptr, noise, out, info, /*append=*/true);
 }
 
 // ---- gradients of logpdf (SURVEY 8f.1) ------------------------------------------------------------

@@ -7,7 +7,7 @@ ARCH="-gencode arch=compute_90a,code=sm_90a"
 FLAGS="$ARCH -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-O2 -Xptxas -v"
 mkdir -p ../../build
 OBJS=""
-for f in assemble gemm_nt ozaki potrf solve p2p cholesky api; do
+for f in assemble gemm_nt ozaki potrf solve append p2p cholesky api; do
   $NVCC $FLAGS -c $f.cu -o ../../build/$f.o 2> ../../build/$f.ptxas.log || { cat ../../build/$f.ptxas.log; exit 1; }
   OBJS="$OBJS ../../build/$f.o"
 done

@@ -171,8 +171,19 @@ void launch_gemv_t(const double* W, int64_t ld, int64_t rows, int64_t cols, cons
 void launch_transpose(const double* in, int64_t ld_in, int64_t rows, int64_t cols, double* out,
                       int64_t ld_out, cudaStream_t st);
 void launch_pack_lower(Packed L, const double* D, int64_t ld, double shift, cudaStream_t st);
-void launch_add_diag(Packed L, const double* d, int64_t n, cudaStream_t st);
 void launch_add_dense_lower(Packed L, const double* D, int64_t ld, int64_t n, cudaStream_t st);
+// appending observations (append.cu)
+// packed S (order Ns) <- M M' + blockdiag(0_r, C) with M = [T; V]: T r x r lower (ld ldt), V (Ns - r) x r (ld ldv),
+// C (Ns - r) x (Ns - r) (ld ldc, lower triangle read).  r = 0 packs C alone.
+void launch_pack_schur(Packed S, int64_t Ns, int r, const double* C, int64_t ldc, const double* T, int64_t ldt,
+                       const double* V, int64_t ldv, cudaStream_t st);
+// C (n x n, ld) += Sigma on and below the diagonal: dense (n x n, ld n), else diag (n), else s2 I
+void launch_add_noise_dense(double* C, int64_t ld, int64_t n, double s2, const double* diag, const double* dense,
+                            cudaStream_t st);
+// joint packed factor J, block columns [0, h / NB): rows [NB j, N1) of the old factor O, then the N2 rows of
+// V (column-major, ld ldv, column = joint column), zero padding below
+void launch_append_relayout(Packed J, Packed O, int64_t N1, int64_t N2, const double* V, int64_t ldv, int64_t h,
+                            cudaStream_t st);
 // VFE gradient helpers (sb_vfe_grad)
 // D (n x n, ld n) <- s I
 void launch_set_scaled_identity(double* D, int64_t n, double s, cudaStream_t st);

@@ -394,11 +394,6 @@ add_dense_lower_kernel(Packed L, const double* __restrict__ D, int64_t ld, int64
     *L.at(r, c) += D[c * ld + r];
 }
 
-__global__ void add_diag_kernel(Packed L, const double* __restrict__ d, int64_t n) {
-    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) *L.at(i, i) += d[i];
-}
-
 __global__ void set_scaled_identity_kernel(double* D, int64_t n, double s) {
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) D[i * n + i] = s;
@@ -471,12 +466,6 @@ void launch_sweep(Packed L, const double* invL, double* b, int S, bool backward,
 void launch_add_dense_lower(Packed L, const double* D, int64_t ld, int64_t n, cudaStream_t st) {
     if (n <= 0) return;
     add_dense_lower_kernel<<<dim3((unsigned)n, (unsigned)((n + 255) / 256)), 256, 0, st>>>(L, D, ld, n);
-    g_launch_count++;
-}
-
-void launch_add_diag(Packed L, const double* d, int64_t n, cudaStream_t st) {
-    if (n <= 0) return;
-    add_diag_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(L, d, n);
     g_launch_count++;
 }
 

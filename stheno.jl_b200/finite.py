@@ -442,14 +442,25 @@ def posterior(fx, y):
         raise TypeError("use posterior(VFE(fz), fx, y)")
     if fx.post is not None:
         # posterior(f_post(x2, s2), y2): sequential conditioning == conditioning the prior on the
-        # stacked observations [x1; x2] with block-diagonal noise (AbstractGPs updates the Cholesky
-        # instead; same distribution).  One joint factorisation on the device.
+        # stacked observations [x1; x2] with block-diagonal noise.  As AbstractGPs' update_chol, p1's
+        # factor is extended on the device (sb_factor_append), not refactorised; p1 itself is unchanged.
         p1 = fx.post
         if not isinstance(p1, PosteriorGP):
             raise NotImplementedError("posterior of an approximate (VFE) posterior is not on the CUDA path")
+        y2 = np.asarray(y, dtype=np.float64)
+        if y2.shape != (len(fx),):
+            raise ValueError("length(y) != length(fx)")
         n1, n2 = npoints(p1.x), len(fx)
         joint = FiniteGP(p1.prior, _stack_inputs(p1.prior, p1.x, fx.x), _stack_noise(n1, p1.noise, n2, fx.noise))
-        return PosteriorGP(joint, np.concatenate([p1.y, np.asarray(y, dtype=np.float64)]))
+        l2 = fx.lowered
+        cross, full = spec_dense(l2, p1.lx), spec_dense(l2, l2)
+        ns = _noise_struct(fx.noise, l2.n)
+        h, info = C.c_void_p(), C.c_int64(0)
+        st = _lib.load().sb_factor_append(p1.fac.ctx.h, p1.fac.h, C.byref(cross), C.byref(full), C.byref(ns),
+                                          C.byref(h), C.byref(info))
+        _lib.check(st, info)
+        joint._factor = _Factor(h, p1.fac.ctx, n1 + n2)
+        return PosteriorGP(joint, np.concatenate([p1.y, y2]))
     return PosteriorGP(fx, y)
 
 

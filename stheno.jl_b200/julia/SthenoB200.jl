@@ -276,17 +276,20 @@ rand(rng::AbstractRNG, fx::B200Finite) = vec(rand(rng, fx, 1))
 
 # ---- exact posterior ------------------------------------------------------------------------------
 struct B200PosteriorGP{T<:B200GPPP} <: AbstractGPs.AbstractGP
-    prior::T; x; F::Factor; α::Vector{Float64}
+    prior::T; x; F::Factor; α::Vector{Float64}; δ::Vector{Float64}
 end
 
-function posterior(fx::B200Finite, y::AbstractVector{<:Real})
-    F = factor(fx); δ = Float64.(y .- host_mean(fx)); α = similar(δ)
+# alpha = C \ δ on the device, stored with the factor it belongs to
+function posterior_from(f::B200GPPP, x, F::Factor, δ::Vector{Float64})
+    α = similar(δ)
     GC.@preserve δ check(ccall((:sb_factor_set_data, LIB), Int32,
         (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}), ctx().h, F.h, δ))
     GC.@preserve α check(ccall((:sb_factor_alpha, LIB), Int32,
         (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}), ctx().h, F.h, α))
-    fp = B200PosteriorGP(fx.f, fx.x, F, α); F.alpha_owner = fp; fp
+    fp = B200PosteriorGP(f, x, F, α, δ); F.alpha_owner = fp; fp
 end
+
+posterior(fx::B200Finite, y::AbstractVector{<:Real}) = posterior_from(fx.f, fx.x, factor(fx), Float64.(y .- host_mean(fx)))
 
 # `posterior` is pure in the reference: a posterior sharing its factor re-installs ITS alpha
 function install_alpha!(fp::B200PosteriorGP)
@@ -357,6 +360,27 @@ function rand(rng::AbstractRNG, fx::B200PostFinite, S::Int)
     out .+ mean(fx)
 end
 rand(rng::AbstractRNG, fx::B200PostFinite) = vec(rand(rng, fx, 1))
+
+# posterior(f_post(x2, Σ2), y2): the posterior of the stacked observations [x; x2] with block-diagonal noise.
+# As AbstractGPs' update_chol, fp's factor is extended on the device (its full block columns are kept), not
+# refactorised; fp itself is unchanged.
+function posterior(fx::B200PostFinite, y::AbstractVector{<:Real})
+    fp = fx.f
+    length(y) == npoints(fx.x) || throw(DimensionMismatch("length(y) != length(fx)"))
+    ps, vs = components(fp.prior, fx.x); po, vo = components(fp.prior, fp.x)
+    cross, k1 = build_spec(ps, vs, po, vo; which=:all)
+    full, k2 = build_spec(ps, vs, ps, vs; which=:all)
+    noise, nd = noise_struct(fx.Σy)
+    h = Ref{Ptr{Cvoid}}(C_NULL); info = Ref{Int64}(0)
+    st = GC.@preserve k1 k2 nd ccall((:sb_factor_append, LIB), Int32,
+        (Ptr{Cvoid}, Ptr{Cvoid}, Ref{SbCovSpec}, Ref{SbCovSpec}, Ref{SbNoise}, Ref{Ptr{Cvoid}}, Ref{Int64}),
+        ctx().h, fp.F.h, cross, full, noise, h, info)
+    check(st, info[])
+    x = BlockData([fp.x, fx.x])
+    F = Factor(h[], npoints(x), nothing); finalizer(destroy!, F)
+    posterior_from(fp.prior, x, F, vcat(fp.δ, Float64.(y .- lowered_mean(fp.prior, fx.x))))
+end
+
 function logpdf(fx::B200PostFinite, y::AbstractVector{<:Real})
     F = factor(fx); δ = Float64.(y .- mean(fx)); out = Ref{Float64}(0.0)
     GC.@preserve δ check(ccall((:sb_logpdf, LIB), Int32,

@@ -56,7 +56,8 @@ EXPORTS = [
     "sb_ctx_destroy", "sb_ctx_timings", "sb_ctx_set_option", "sb_ctx_mark", "sb_ctx_elapsed_ms", "sb_owner_of_block",
     "sb_owned_trailing_tiles", "sb_row_chunk", "sb_cov_dense", "sb_cov_diag", "sb_factor_create",
     "sb_factor_destroy", "sb_factor_logdet", "sb_logpdf", "sb_factor_set_data", "sb_factor_alpha",
-    "sb_factor_set_alpha", "sb_predict", "sb_predict_cov", "sb_predict_factor", "sb_rand", "sb_factor_get_L",
+    "sb_factor_set_alpha", "sb_predict", "sb_predict_cov", "sb_predict_factor", "sb_factor_append", "sb_rand",
+    "sb_factor_get_L",
     "sb_vfe_create", "sb_vfe_predict", "sb_vfe_predict_cov", "sb_vfe_destroy",
     "sb_factor_export_size", "sb_factor_export", "sb_factor_import", "sb_logpdf_grad", "sb_vfe_grad",
 ]
@@ -113,6 +114,7 @@ def load():
         "sb_predict": [vp, vp, P(sb_covspec), P(sb_covspec), vp, vp],
         "sb_predict_cov": [vp, vp, P(sb_covspec), P(sb_covspec), vp],
         "sb_predict_factor": [vp, vp, P(sb_covspec), P(sb_covspec), P(sb_noise), P(vp), P(i64)],
+        "sb_factor_append": [vp, vp, P(sb_covspec), P(sb_covspec), P(sb_noise), P(vp), P(i64)],
         "sb_rand": [vp, vp, vp, i32, vp],
         "sb_factor_get_L": [vp, vp, vp],
         "sb_logpdf_grad": [vp, vp, P(sb_covspec), vp, vp],
