@@ -13,3 +13,7 @@ for f in assemble gemm_nt ozaki potrf solve append p2p cholesky api; do
 done
 $NVCC $ARCH -shared -o ../libstheno_b200.so $OBJS -lcudart -ldl
 echo "built $(cd ..; pwd)/libstheno_b200.so"
+# test-only probe: C entry points onto the kernel launchers (tests/test_gpu_kernels.py)
+$NVCC $ARCH -O2 -std=c++17 -Xcompiler -fPIC -cudart shared -shared -o ../../build/libsb_probe.so \
+  ../../tests/kernels/probe.cu -L.. -lstheno_b200 -Xlinker -rpath,'$ORIGIN/../stheno.jl_b200'
+echo "built $(cd ../../build; pwd)/libsb_probe.so"
