@@ -71,9 +71,11 @@ struct DevSpec {
     std::vector<double*> arr;
     std::vector<BlockDev> blocks;
     int64_t nrows = 0, ncols = 0;
+    bool diag = false;  // paired points: every block is square and evaluated on its diagonal only
 
-    int32_t build(const sb_covspec* spec, cudaStream_t st, bool diag) {
+    int32_t build(const sb_covspec* spec, cudaStream_t st, bool paired) {
         SB_CHECK(spec != nullptr, "null covspec");
+        diag = paired;
         nrows = spec->nrows;
         ncols = spec->ncols;
         SB_CHECK(nrows >= 0 && ncols >= 0, "negative matrix size");
@@ -142,9 +144,9 @@ struct DevSpec {
     }
 };
 
-// keep only rows [lo, hi) of every block (and, for paired/diag specs, the same range of columns);
-// rows are re-based to lo.  Used to shard the posterior's test points across ranks.
-void clip_rows(DevSpec& ds, int64_t lo, int64_t hi, bool diag) {
+// the blocks of rows [lo, hi) of a plan (and, for paired/diag specs, the same range of columns), re-based to
+// row lo.  Used for the row chunks of the VFE stream and to shard the posterior's test points across ranks.
+std::vector<BlockDev> clip_rows(const DevSpec& ds, int64_t lo, int64_t hi) {
     std::vector<BlockDev> out;
     for (BlockDev b : ds.blocks) {
         int64_t r0 = b.row0 > lo ? b.row0 : lo;
@@ -154,19 +156,25 @@ void clip_rows(DevSpec& ds, int64_t lo, int64_t hi, bool diag) {
         for (int t = 0; t < b.nterms; t++) {
             b.t[t].zl += off * b.t[t].dim;
             if (b.t[t].sl) b.t[t].sl += off;
-            if (diag) {
+            if (ds.diag) {
                 b.t[t].zr += off * b.t[t].dim;
                 if (b.t[t].sr) b.t[t].sr += off;
             }
         }
         b.row0 = r0 - lo;
         b.nrows = r1 - r0;
-        if (diag) { b.col0 = b.row0; b.ncols = b.nrows; }
+        if (ds.diag) { b.col0 = b.row0; b.ncols = b.nrows; }
         out.push_back(b);
     }
-    ds.blocks.swap(out);
-    ds.nrows = hi - lo;
-    if (diag) ds.ncols = hi - lo;
+    return out;
+}
+
+// rank's contiguous share [lo, hi) of ns rows split over world ranks in chunks of `chunk` rows
+struct RowChunk { int64_t lo, hi, chunk; };
+RowChunk row_chunk(int64_t ns, int rank, int world) {
+    const int64_t chunk = (ns + world - 1) / world;
+    const int64_t lo = rank * chunk < ns ? rank * chunk : ns;
+    return {lo, lo + chunk < ns ? lo + chunk : ns, chunk};
 }
 
 void begin_call(sb_ctx* c) {
@@ -174,17 +182,51 @@ void begin_call(sb_ctx* c) {
     c->ev_used = 0;
 }
 
-void count_launches(sb_ctx* c, int64_t before) { c->tm.kernel_launches += g_launch_count - before; }
+// The sb_timings fields an ABI call's stream time adds to: none, total_ms, or predict_ms and total_ms
+enum class Timed { no, total, predict };
 
-// dense assembly of a (possibly padded) nrows x ncols matrix with leading dimension ld
-int32_t assemble_dense(sb_ctx* c, DevSpec& ds, double* out, int64_t ld) {
-    for (auto& b : ds.blocks) launch_assemble_dense(b, OutDense{out, ld}, c->stream);
+// Bracket of an ABI call that launches kernels: it starts the call (begin_call) and, on the success path, end()
+// adds the call's kernel launches to kernel_launches and its stream time to the fields `timed` names.  Helpers
+// inside a call do neither, so every launch is counted once.
+struct Call {
+    sb_ctx* c;
+    Timed timed;
+    int64_t before = g_launch_count;
+    cudaEvent_t t0 = nullptr;
+    Call(sb_ctx* ctx, Timed t = Timed::no) : c(ctx), timed(t) {
+        begin_call(c);
+        if (timed != Timed::no) {
+            t0 = c->next_event();
+            cudaEventRecord(t0, c->stream);
+        }
+    }
+    int32_t end() {
+        if (timed != Timed::no) {
+            cudaEvent_t t1 = c->next_event();
+            cudaEventRecord(t1, c->stream);
+            SB_CUDA(cudaEventSynchronize(t1));
+            float ms = 0;
+            cudaEventElapsedTime(&ms, t0, t1);
+            if (timed == Timed::predict) c->tm.predict_ms += ms;
+            c->tm.total_ms += ms;
+        }
+        c->tm.kernel_launches += g_launch_count - before;
+        return SB_OK;
+    }
+};
+
+// zero the padded matrix out (ld x ncols) and assemble blocks into it
+int32_t assemble_dense(sb_ctx* c, const std::vector<BlockDev>& blocks, double* out, int64_t ld, int64_t ncols) {
+    SB_CUDA(cudaMemsetAsync(out, 0, (size_t)ld * ncols * sizeof(double), c->stream));
+    for (auto& b : blocks) launch_assemble_dense(b, OutDense{out, ld}, c->stream);
     SB_CUDA(cudaGetLastError());
     return SB_OK;
 }
 
-int32_t assemble_diag(sb_ctx* c, DevSpec& ds, double* out) {
-    for (auto& b : ds.blocks) launch_assemble_diag(b, out, c->stream);
+// zero the vector out (n entries) and assemble the diagonal of the paired blocks into it
+int32_t assemble_diag(sb_ctx* c, const std::vector<BlockDev>& blocks, double* out, int64_t n) {
+    SB_CUDA(cudaMemsetAsync(out, 0, n * sizeof(double), c->stream));
+    for (auto& b : blocks) launch_assemble_diag(b, out, c->stream);
     SB_CUDA(cudaGetLastError());
     return SB_OK;
 }
@@ -319,9 +361,9 @@ int64_t sb_owned_trailing_tiles(int64_t nblk, int64_t k, int32_t rank, int32_t w
 
 int32_t sb_row_chunk(int64_t ns, int32_t rank, int32_t world, int64_t* lo, int64_t* hi) {
     SB_CHECK(lo && hi && world >= 1 && rank >= 0 && rank < world && ns >= 0, "bad argument");
-    int64_t chunk = (ns + world - 1) / world;
-    *lo = rank * chunk < ns ? rank * chunk : ns;
-    *hi = *lo + chunk < ns ? *lo + chunk : ns;
+    const RowChunk rc = row_chunk(ns, rank, world);
+    *lo = rc.lo;
+    *hi = rc.hi;
     return SB_OK;
 }
 
@@ -344,39 +386,33 @@ int32_t sb_ctx_elapsed_ms(sb_ctx* c, int32_t a, int32_t b, double* ms) {
 
 int32_t sb_cov_dense(sb_ctx* c, const sb_covspec* spec, void* K_out) {
     SB_CHECK(c && spec && K_out, "null argument");
-    begin_call(c);
-    int64_t before = g_launch_count;
+    Call call(c);
     DevSpec ds(c);
     SB_TRY(ds.build(spec, c->stream, false));
     DevBuf K(c);
     size_t bytes = (size_t)ds.nrows * ds.ncols * sizeof(double);
     SB_TRY(K.alloc(bytes));
-    SB_CUDA(cudaMemsetAsync(K.p, 0, bytes, c->stream));
     Timer t(c, true);
     cudaEvent_t t0 = t.mark(c->stream);
-    SB_TRY(assemble_dense(c, ds, K.d(), ds.nrows));
+    SB_TRY(assemble_dense(c, ds.blocks, K.d(), ds.nrows, ds.ncols));
     t.add(t0, t.mark(c->stream), &c->tm.assemble_ms);
     SB_CUDA(cudaMemcpyAsync(K_out, K.p, bytes, cudaMemcpyDefault, c->stream));
     SB_CUDA(cudaStreamSynchronize(c->stream));
     t.collect();
-    count_launches(c, before);
-    return SB_OK;
+    return call.end();
 }
 
 int32_t sb_cov_diag(sb_ctx* c, const sb_covspec* spec, void* out) {
     SB_CHECK(c && spec && out, "null argument");
-    begin_call(c);
-    int64_t before = g_launch_count;
+    Call call(c);
     DevSpec ds(c);
     SB_TRY(ds.build(spec, c->stream, true));
     DevBuf v(c);
     SB_TRY(v.alloc(ds.nrows * sizeof(double)));
-    SB_CUDA(cudaMemsetAsync(v.p, 0, ds.nrows * sizeof(double), c->stream));
-    SB_TRY(assemble_diag(c, ds, v.d()));
+    SB_TRY(assemble_diag(c, ds.blocks, v.d(), ds.nrows));
     SB_CUDA(cudaMemcpyAsync(out, v.p, ds.nrows * sizeof(double), cudaMemcpyDefault, c->stream));
     SB_CUDA(cudaStreamSynchronize(c->stream));
-    count_launches(c, before);
-    return SB_OK;
+    return call.end();
 }
 
 int32_t sb_factor_destroy(sb_factor* f) {
@@ -431,34 +467,36 @@ static int32_t factor_alloc(sb_ctx* c, int64_t N, std::unique_ptr<sb_factor>& ou
     return SB_OK;
 }
 
-// run the Cholesky on an assembled packed matrix and collect info / logdet
-static int32_t factor_finish(sb_ctx* c, sb_factor* f, int64_t* info, bool force_local) {
-    SB_TRY(cholesky_packed(c, f, force_local));
-    const int64_t nblk = f->L.nblk();
-    long long h_info = 0;
-    std::vector<double> ld(nblk);
-    SB_CUDA(cudaMemcpy(&h_info, f->info_dev, sizeof(long long), cudaMemcpyDeviceToHost));
-    SB_CUDA(cudaMemcpy(ld.data(), f->logdet_blk, nblk * sizeof(double), cudaMemcpyDeviceToHost));
-    if (h_info != 0) {
-        if (info) *info = (int64_t)h_info;
-        sb::set_error("matrix is not positive definite; Cholesky factorization failed at pivot " +
-                      std::to_string(h_info));
-        return SB_ERR_NOT_POSDEF;
-    }
+// f->logdet from the per-block log-pivots, summed on the host in block order
+static int32_t sum_logdet(sb_ctx* c, sb_factor* f) {
+    std::vector<double> ld(f->L.nblk());
+    SB_CUDA(cudaMemcpyAsync(ld.data(), f->logdet_blk, ld.size() * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    SB_CUDA(cudaStreamSynchronize(c->stream));
     double sum = 0.0;
     for (double v : ld) sum += v;
     f->logdet = sum;
     return SB_OK;
 }
 
+// run the Cholesky on an assembled packed matrix and collect info / logdet
+static int32_t factor_finish(sb_ctx* c, sb_factor* f, int64_t* info, bool force_local) {
+    SB_TRY(cholesky_packed(c, f, force_local));
+    long long h_info = 0;
+    SB_CUDA(cudaMemcpy(&h_info, f->info_dev, sizeof(long long), cudaMemcpyDeviceToHost));
+    if (h_info != 0) {
+        if (info) *info = (int64_t)h_info;
+        sb::set_error("matrix is not positive definite; Cholesky factorization failed at pivot " +
+                      std::to_string(h_info));
+        return SB_ERR_NOT_POSDEF;
+    }
+    return sum_logdet(c, f);
+}
+
 static int32_t factor_create_impl(sb_ctx* c, const sb_covspec* spec, const sb_noise* noise,
                                   std::unique_ptr<sb_factor>& out, int64_t* info, bool force_local) {
     SB_CHECK(spec->symmetric == 1 && spec->nrows == spec->ncols, "factor needs a symmetric square spec");
     SB_CHECK(spec->nrows > 0, "empty matrix");
-    int64_t before = g_launch_count;
     if (info) *info = 0;
-    cudaEvent_t t0 = c->next_event(), t1 = c->next_event();
-    cudaEventRecord(t0, c->stream);
 
     DevSpec ds(c);
     SB_TRY(ds.build(spec, c->stream, false));
@@ -490,12 +528,6 @@ static int32_t factor_create_impl(sb_ctx* c, const sb_covspec* spec, const sb_no
     SB_CUDA(cudaGetLastError());
     SB_TRY(factor_finish(c, f.get(), info, force_local));
     t.collect();
-    cudaEventRecord(t1, c->stream);
-    cudaEventSynchronize(t1);
-    float ms = 0;
-    cudaEventElapsedTime(&ms, t0, t1);
-    c->tm.total_ms += ms;
-    count_launches(c, before);
     out = std::move(f);
     return SB_OK;
 }
@@ -503,11 +535,12 @@ static int32_t factor_create_impl(sb_ctx* c, const sb_covspec* spec, const sb_no
 int32_t sb_factor_create(sb_ctx* c, const sb_covspec* spec, const sb_noise* noise, sb_factor** out,
                          int64_t* info) {
     SB_CHECK(c && spec && out, "null argument");
-    begin_call(c);
+    Call call(c, Timed::total);
     std::unique_ptr<sb_factor> f;
-    const int32_t st = factor_create_impl(c, spec, noise, f, info, false);
+    *out = nullptr;
+    SB_TRY(factor_create_impl(c, spec, noise, f, info, false));
     *out = f.release();
-    return st;
+    return call.end();
 }
 
 // ---- factor checkpoint: export / import (SURVEY 8f.4) -------------------------------------------
@@ -583,8 +616,7 @@ int32_t sb_factor_logdet(sb_ctx*, sb_factor* f, double* out) {
 
 int32_t sb_logpdf(sb_ctx* c, sb_factor* f, const void* delta, int32_t S, double* out) {
     SB_CHECK(c && f && delta && out && S >= 1, "bad argument");
-    begin_call(c);
-    int64_t before = g_launch_count;
+    Call call(c);
     DevBuf b(c), q(c);
     SB_TRY(b.alloc((size_t)f->Np * S * sizeof(double)));
     SB_TRY(q.alloc(S * sizeof(double)));
@@ -606,14 +638,12 @@ int32_t sb_logpdf(sb_ctx* c, sb_factor* f, const void* delta, int32_t S, double*
     t.collect();
     const double log2pi = 1.8378770664093454835606594728112;
     for (int s = 0; s < S; s++) out[s] = -((double)f->N * log2pi + f->logdet + hq[s]) / 2.0;
-    count_launches(c, before);
-    return SB_OK;
+    return call.end();
 }
 
 int32_t sb_factor_set_data(sb_ctx* c, sb_factor* f, const void* delta) {
     SB_CHECK(c && f && delta, "null argument");
-    begin_call(c);
-    int64_t before = g_launch_count;
+    Call call(c);
     SB_TRY(upload_padded(c, delta, f->N, f->Np, 1, f->alpha));
     Timer t(c, true);
     cudaEvent_t t0 = t.mark(c->stream);
@@ -635,8 +665,7 @@ int32_t sb_factor_set_data(sb_ctx* c, sb_factor* f, const void* delta) {
     SB_CUDA(cudaStreamSynchronize(c->stream));
     t.collect();
     f->has_alpha = true;
-    count_launches(c, before);
-    return SB_OK;
+    return call.end();
 }
 
 // posterior(fx, y) is a pure function in the reference (AbstractGPs PosteriorGP holds its own
@@ -659,38 +688,39 @@ int32_t sb_factor_alpha(sb_ctx* c, sb_factor* f, void* alpha_out) {
     return SB_OK;
 }
 
-// workspace of the int8 Ozaki matrix-TRSM sweep: digit planes / scales / tensor maps of the X panels
-struct OzSweepWs {
-    DevBuf planes, scale, expo;
+// Workspace of trsm_sweep for sweeps of up to `rows` rows: the X panels (rows x 512) and, only when asked for, the
+// int8 digit planes, scales and tensor maps of X that the int8 Ozaki update reads
+struct SweepWs {
+    DevBuf X, planes, scale, expo;
     OzMaps maps;
-    int64_t rows = 0;
-    bool ready = false;
-    explicit OzSweepWs(sb_ctx* c) : planes(c), scale(c), expo(c) {}
-    int32_t init(int64_t rows_p) {
-        rows = rows_p;
-        SB_TRY(planes.alloc(oz_planes_bytes(rows_p)));
-        SB_TRY(scale.alloc(rows_p * sizeof(double)));
-        SB_TRY(expo.alloc(rows_p * sizeof(int)));
-        if (oz_make_maps(reinterpret_cast<signed char*>(planes.p), rows_p, &maps) != 0) {
+    int64_t plane_rows = 0;  // 0: no planes, every sweep runs its big update on DMMA
+    explicit SweepWs(sb_ctx* c) : X(c), planes(c), scale(c), expo(c) {}
+    int32_t init(int64_t rows, bool int8) {
+        SB_TRY(X.alloc((size_t)rows * OUTER_BLOCKS * NB * sizeof(double)));
+        return int8 ? add_planes(rows) : SB_OK;
+    }
+    int32_t add_planes(int64_t rows) {
+        plane_rows = rows;
+        SB_TRY(planes.alloc(oz_planes_bytes(rows)));
+        SB_TRY(scale.alloc(rows * sizeof(double)));
+        SB_TRY(expo.alloc(rows * sizeof(int)));
+        if (oz_make_maps(reinterpret_cast<signed char*>(planes.p), rows, &maps) != 0) {
             sb::set_error("cuTensorMapEncodeTiled failed for the X digit planes");
             return SB_ERR_CUDA;
         }
-        ready = true;
         return SB_OK;
     }
 };
-constexpr int SWEEP_COLS = OUTER_BLOCKS * NB;  // columns of the Xk workspace (rows_p x 512)
 
 // W <- W L^{-T} (rows_p x Np, ld rows_p): right-looking block forward substitution, tensor-core
 // products only.  keep: write the result back into W; acc != null: acc[r] += sum_c result[r,c]^2.
-// Xk: rows_p x 512 workspace.  Each outer step solves 4 block columns (small in-step DMMA products)
-// and then applies them to the rest of W in one big update with K = 512, which reads and writes the
-// remaining columns of W once per 4 block columns.  That update runs on DMMA, or on the int8 Ozaki
-// kernel for an int8-Ozaki factor (f->oz) given its workspace.
-static int32_t trsm_sweep(sb_ctx* c, sb_factor* f, double* W, int64_t rows_p, double* Xk, bool keep, double* acc,
-                          OzSweepWs* ws = nullptr) {
+// Each outer step solves 4 block columns into ws.X (small in-step DMMA products) and then applies
+// them to the rest of W in one big update with K = 512, which reads and writes the remaining columns
+// of W once per 4 block columns.  That update runs on the int8 Ozaki kernel for an int8-Ozaki factor
+// (f->oz) when ws has digit planes, and on DMMA otherwise.
+static int32_t trsm_sweep(sb_ctx* c, sb_factor* f, double* W, int64_t rows_p, SweepWs& ws, bool keep, double* acc) {
     const int64_t nblk = f->L.nblk(), Np = f->Np;
-    const bool oz = f->oz && ws && ws->ready;
+    const bool oz = f->oz && ws.plane_rows > 0;
     const int64_t las[OUTER_BLOCKS] = {rows_p, rows_p, rows_p, rows_p};
     for (int64_t k0 = 0; k0 < nblk; k0 += OUTER_BLOCKS) {
         const int nq = outer_width(nblk, k0);
@@ -698,7 +728,7 @@ static int32_t trsm_sweep(sb_ctx* c, sb_factor* f, double* W, int64_t rows_p, do
         for (int q = 0; q < nq; q++) {
             const int64_t kq = k0 + q;
             double* Wq = W + kq * NB * rows_p;
-            double* Xq = Xk + (int64_t)q * NB * rows_p;
+            double* Xq = ws.X.d() + (int64_t)q * NB * rows_p;
             X[q] = Xq;
             if (q > 0) {  // bring block column kq up to date with the X panels of this outer step
                 const double* Bs[OUTER_BLOCKS]; int64_t lbs[OUTER_BLOCKS];
@@ -723,10 +753,10 @@ static int32_t trsm_sweep(sb_ctx* c, sb_factor* f, double* W, int64_t rows_p, do
             sx.base[q] = X[q]; sx.ld[q] = rows_p; sx.rbs[q] = NB;
             sl.base[q] = f->L.blk(jt, k0 + q); sl.ld[q] = f->L.ld(k0 + q); sl.rbs[q] = NB;
         }
-        launch_oz_slice(sx, 0, rows_p / NB, 0, ws->rows, ws->scale.d(), reinterpret_cast<int*>(ws->expo.p),
-                        reinterpret_cast<signed char*>(ws->planes.p), c->stream);
+        launch_oz_slice(sx, 0, rows_p / NB, 0, ws.plane_rows, ws.scale.d(), reinterpret_cast<int*>(ws.expo.p),
+                        reinterpret_cast<signed char*>(ws.planes.p), c->stream);
         launch_oz_slice(sl, 0, m / NB, jt * (int64_t)NB, Np, f->oz_scale[0], f->oz_expo[0], f->oz_planes[0], c->stream);
-        if (launch_gemm_ozaki(W + jt * NB * rows_p, rows_p, rows_p, m, nq, &ws->maps, ws->scale.d(), 0, &f->oz_maps[0],
+        if (launch_gemm_ozaki(W + jt * NB * rows_p, rows_p, rows_p, m, nq, &ws.maps, ws.scale.d(), 0, &f->oz_maps[0],
                               f->oz_scale[0], jt * (int64_t)NB, c->stream) != 0) {
             sb::set_error("int8 Ozaki sweep kernel could not be launched");
             return SB_ERR_CUDA;
@@ -746,7 +776,6 @@ static int32_t factor_splice(sb_ctx* c, const sb_factor* f, const sb_factor* S, 
     std::unique_ptr<sb_factor> g;
     SB_TRY(factor_alloc(c, h + S->N, g));
     SB_CHECK(g->Np - h == S->Np, "append: Schur factor does not match the joint layout");
-    const int64_t nblk = g->L.nblk();
     launch_append_relayout(g->L, f->L, f->N, N2, V, ldv, h, c->stream);
     SB_CUDA(cudaMemcpyAsync(g->L.base + g->L.off(nh), S->L.base, (size_t)S->L.total() * sizeof(double),
                             cudaMemcpyDeviceToDevice, c->stream));
@@ -755,49 +784,115 @@ static int32_t factor_splice(sb_ctx* c, const sb_factor* f, const sb_factor* S, 
     SB_CUDA(cudaMemcpyAsync(g->logdet_blk, f->logdet_blk, nh * sizeof(double), cudaMemcpyDeviceToDevice, c->stream));
     SB_CUDA(cudaMemcpyAsync(g->logdet_blk + nh, S->logdet_blk, S->logdet_blk.bytes, cudaMemcpyDeviceToDevice, c->stream));
     SB_CUDA(cudaGetLastError());
-    std::vector<double> ld(nblk);
-    SB_CUDA(cudaMemcpyAsync(ld.data(), g->logdet_blk, nblk * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-    SB_CUDA(cudaStreamSynchronize(c->stream));
-    double sum = 0.0;   // summed in block order, as factor_finish does for a fresh factor
-    for (double v : ld) sum += v;
-    g->logdet = sum;
+    SB_TRY(sum_logdet(c, g.get()));
     out = std::move(g);
     return SB_OK;
 }
 
-// shared body of sb_predict / sb_predict_cov / sb_predict_factor / sb_factor_append
-static int32_t predict_impl(sb_ctx* c, sb_factor* f, const sb_covspec* cross,
-                            const sb_covspec* prior, bool full_cov, void* mean_out, void* var_out,
-                            void* cov_out, const sb_noise* post_noise = nullptr, sb_factor** fac_out = nullptr,
-                            int64_t* info = nullptr, bool append = false) {
-    begin_call(c);
-    int64_t before = g_launch_count;
+// Posterior step (a): rows [lo, hi) of a cross spec (K_{*f}, or K_{*u} for VFE) assembled into the zero-padded W
+// (rows_p x cols, ld rows_p), then swept by triangular factors, W <- W L^{-T}, with keep and/or a row-sum-of-squares
+// accumulator (trsm_sweep).  The caller sizes the sweep workspace (ws.init) for the factors it sweeps by.
+struct CrossRows {
+    sb_ctx* c;
+    int64_t rows_p = 0;
+    DevBuf W;
+    SweepWs ws;
+    explicit CrossRows(sb_ctx* ctx) : c(ctx), W(ctx), ws(ctx) {}
+    int32_t assemble(const DevSpec& cross, int64_t lo, int64_t hi, int64_t cols) {
+        rows_p = round_up(hi > lo ? hi - lo : 1, NB);
+        SB_TRY(W.alloc((size_t)rows_p * cols * sizeof(double)));
+        return assemble_dense(c, clip_rows(cross, lo, hi), W.d(), rows_p, cols);
+    }
+    int32_t sweep(sb_factor* f, bool keep, double* acc) { return trsm_sweep(c, f, W.d(), rows_p, ws, keep, acc); }
+};
+
+// Posterior step (c): Cm = prior - W W^T (rows_p x rows_p, ld rows_p) for the Ns test points, with W = K_{*f} L^{-T}
+// kept in x.W (the append splices its columns into the joint factor)
+struct PosteriorCov {
+    DevSpec dc, dp;
+    CrossRows x;
+    DevBuf Cm;
+    int64_t Ns = 0;
+    explicit PosteriorCov(sb_ctx* c) : dc(c), dp(c), x(c), Cm(c) {}
+    int32_t build(sb_ctx* c, sb_factor* f, const sb_covspec* cross, const sb_covspec* prior) {
+        Ns = cross->nrows;
+        SB_TRY(dc.build(cross, c->stream, false));
+        SB_CHECK(prior->nrows == Ns, "prior spec size mismatch");
+        SB_TRY(dp.build(prior, c->stream, false));
+        SB_TRY(x.assemble(dc, 0, Ns, f->Np));
+        SB_TRY(x.ws.init(x.rows_p, f->oz));
+        SB_TRY(x.sweep(f, /*keep=*/true, nullptr));
+        const int64_t Nsp = x.rows_p;
+        SB_TRY(Cm.alloc((size_t)Nsp * Nsp * sizeof(double)));
+        SB_TRY(assemble_dense(c, dp.blocks, Cm.d(), Nsp, Nsp));
+        launch_gemm_nt(x.W.d(), Nsp, x.W.d(), Nsp, Cm.d(), Nsp, Nsp, Nsp, f->Np, -1.0, 1.0, c->stream);
+        SB_CUDA(cudaGetLastError());
+        return SB_OK;
+    }
+};
+
+// Posterior step (d): the Cholesky factor of S = (Cm + noise, with the Schur complement of f's first h rows),
+// of order r + Ns.  h = r = 0 (sb_predict_factor): S is the noisy posterior covariance.  h = NB floor(N / NB),
+// r = N - h (sb_factor_append): S is the Schur complement of f's head in the joint matrix, whose first r rows
+// are the old rows of f's partial last block, and its factor is spliced behind that head (factor_splice).  A
+// failing pivot is reported in the order of the joint matrix.
+static int32_t factor_posterior(sb_ctx* c, sb_factor* f, PosteriorCov& pc, const sb_noise* noise, int64_t h, int r,
+                                sb_factor** out, int64_t* info) {
+    const int64_t Ns = pc.Ns, Nsp = pc.x.rows_p;
+    DevBuf nd(c);
+    const bool pn_dense = noise && noise->dense, pn_diag = noise && noise->diag;
+    if (pn_dense || pn_diag) {
+        const size_t n = pn_dense ? (size_t)Ns * Ns : (size_t)Ns;
+        SB_TRY(nd.alloc(n * sizeof(double)));
+        SB_CUDA(cudaMemcpyAsync(nd.p, pn_dense ? noise->dense : noise->diag, n * sizeof(double), cudaMemcpyDefault,
+                                c->stream));
+    }
+    launch_add_noise_dense(pc.Cm.d(), Nsp, Ns, noise ? noise->sigma2 : 0.0, pn_diag && !pn_dense ? nd.d() : nullptr,
+                           pn_dense ? nd.d() : nullptr, c->stream);
+    std::unique_ptr<sb_factor> fn;
+    SB_TRY(factor_alloc(c, r + Ns, fn));
+    launch_pack_schur(fn->L, r + Ns, r, pc.Cm.d(), Nsp, r ? f->L.blk(h / NB, h / NB) : nullptr, f->L.ld(h / NB),
+                      r ? pc.x.W.d() + h * Nsp : nullptr, Nsp, c->stream);
+    launch_fill_padding(fn->L, r + Ns, c->stream);
+    int64_t info_s = 0;
+    const int32_t st = factor_finish(c, fn.get(), &info_s, /*force_local=*/true);
+    if (st == SB_ERR_NOT_POSDEF) {   // S's pivot index, in the order of the joint matrix
+        if (info) *info = h + info_s;
+        if (h > 0)
+            sb::set_error("matrix is not positive definite; Cholesky factorization failed at pivot " +
+                          std::to_string(h + info_s));
+    }
+    SB_TRY(st);
+    if (h > 0) {
+        std::unique_ptr<sb_factor> joint;
+        SB_TRY(factor_splice(c, f, fn.get(), pc.x.W.d(), Nsp, Ns, joint));
+        fn = std::move(joint);
+    }
+    *out = fn.release();
+    return SB_OK;
+}
+
+// Posterior step (b): mean and/or var at the test points.  Multi-GPU: every rank holds the complete factor, so the
+// test points are sharded by rows (contiguous chunks, as sb_row_chunk) with no communication until the final
+// all-gather of mean / var.
+int32_t sb_predict(sb_ctx* c, sb_factor* f, const sb_covspec* cross, const sb_covspec* prior_diag,
+                   void* mean_out, void* var_out) {
+    SB_CHECK(c && f && cross, "null argument");
     SB_CHECK(cross->ncols == f->N, "cross spec must be N* x N");
+    Call call(c, Timed::predict);
     const int64_t Ns_all = cross->nrows;
     if (Ns_all == 0) return SB_OK;
-    // multi-GPU: every rank holds the complete factor, so the test points are sharded by rows
-    // (contiguous chunks) with no communication until the final all-gather of mean / var.
-    const bool shard = c->world > 1 && !full_cov;
-    const int64_t chunk = shard ? (Ns_all + c->world - 1) / c->world : Ns_all;
-    const int64_t lo = shard ? (c->rank * chunk < Ns_all ? c->rank * chunk : Ns_all) : 0;
-    const int64_t hi = shard ? (lo + chunk < Ns_all ? lo + chunk : Ns_all) : Ns_all;
-    const int64_t Ns = hi - lo, Nsp = round_up(Ns > 0 ? Ns : 1, NB), Np = f->Np;
-    const int64_t nblk = f->L.nblk();
-    const bool need_var = var_out != nullptr || full_cov;
     SB_CHECK(!mean_out || f->has_alpha, "posterior mean requested before sb_factor_set_data");
-    cudaEvent_t t0 = c->next_event(), t1 = c->next_event();
-    cudaEventRecord(t0, c->stream);
+    const bool shard = c->world > 1;
+    const RowChunk rc = row_chunk(Ns_all, c->rank, c->world);
+    const int64_t Ns = rc.hi - rc.lo, chunk = rc.chunk, Np = f->Np;
 
     DevSpec dc(c), dp(c);
     SB_TRY(dc.build(cross, c->stream, false));
-    if (need_var) {
-        SB_CHECK(prior != nullptr, "prior spec required for var/cov");
-        SB_CHECK(prior->nrows == Ns_all, "prior spec size mismatch");
-        SB_TRY(dp.build(prior, c->stream, !full_cov));
-    }
-    if (shard) {
-        clip_rows(dc, lo, hi, false);
-        if (need_var) clip_rows(dp, lo, hi, true);
+    if (var_out) {
+        SB_CHECK(prior_diag != nullptr, "prior spec required for var/cov");
+        SB_CHECK(prior_diag->nrows == Ns_all, "prior spec size mismatch");
+        SB_TRY(dp.build(prior_diag, c->stream, true));
     }
     DevBuf gath(c);  // [2][world][chunk] gather buffer (mean, var) when sharded
     if (shard) SB_TRY(gath.alloc((size_t)2 * (c->world + 1) * chunk * sizeof(double)));
@@ -806,85 +901,32 @@ static int32_t predict_impl(sb_ctx* c, sb_factor* f, const sb_covspec* cross,
     double* g_recv_m = shard ? gath.d() + 2 * chunk : nullptr;           // world*chunk
     double* g_recv_v = shard ? gath.d() + 2 * chunk + (size_t)c->world * chunk : nullptr;
     if (shard) SB_CUDA(cudaMemsetAsync(gath.p, 0, (size_t)2 * (c->world + 1) * chunk * sizeof(double), c->stream));
-    DevBuf W(c), Xk(c), mean(c), acc(c), pd(c);
-    SB_TRY(W.alloc((size_t)Nsp * Np * sizeof(double)));
-    SB_CUDA(cudaMemsetAsync(W.p, 0, (size_t)Nsp * Np * sizeof(double), c->stream));
-    SB_TRY(assemble_dense(c, dc, W.d(), Nsp));
+    CrossRows x(c);
+    SB_TRY(x.assemble(dc, rc.lo, rc.hi, Np));
+    const int64_t Nsp = x.rows_p;
+    DevBuf mean(c), acc(c), pd(c);
     if (mean_out) {
         SB_TRY(mean.alloc(Nsp * sizeof(double)));
-        launch_gemv_n(W.d(), Nsp, Nsp, Np, f->alpha, mean.d(), c->stream);
+        launch_gemv_n(x.W.d(), Nsp, Nsp, Np, f->alpha, mean.d(), c->stream);
         if (shard) {
             if (Ns > 0) SB_CUDA(cudaMemcpyAsync(g_send_m, mean.p, Ns * sizeof(double), cudaMemcpyDeviceToDevice, c->stream));
         } else {
             SB_CUDA(cudaMemcpyAsync(mean_out, mean.p, Ns * sizeof(double), cudaMemcpyDefault, c->stream));
         }
     }
-    if (need_var) {
-        SB_TRY(Xk.alloc((size_t)Nsp * SWEEP_COLS * sizeof(double)));
+    if (var_out) {
         SB_TRY(acc.alloc(Nsp * sizeof(double)));
         SB_CUDA(cudaMemsetAsync(acc.p, 0, Nsp * sizeof(double), c->stream));
-        // V^T = W L^{-T}: block forward substitution from the right, tensor-core products only
-        OzSweepWs ws(c);
-        if (f->oz) SB_TRY(ws.init(Nsp));
-        SB_TRY(trsm_sweep(c, f, W.d(), Nsp, Xk.d(), /*keep=*/full_cov, full_cov ? nullptr : acc.d(), &ws));
-        if (!full_cov) {
-            SB_TRY(pd.alloc(Nsp * sizeof(double)));
-            SB_CUDA(cudaMemsetAsync(pd.p, 0, Nsp * sizeof(double), c->stream));
-            SB_TRY(assemble_diag(c, dp, pd.d()));
-            launch_sub(pd.d(), pd.d(), acc.d(), Ns, c->stream);
-            if (var_out && shard) {
-                if (Ns > 0) SB_CUDA(cudaMemcpyAsync(g_send_v, pd.p, Ns * sizeof(double), cudaMemcpyDeviceToDevice, c->stream));
-            } else if (var_out) {
-                SB_CUDA(cudaMemcpyAsync(var_out, pd.p, Ns * sizeof(double), cudaMemcpyDefault, c->stream));
-            }
+        // rows of V^T = W L^{-T}: block forward substitution from the right, tensor-core products only
+        SB_TRY(x.ws.init(Nsp, f->oz));
+        SB_TRY(x.sweep(f, /*keep=*/false, acc.d()));
+        SB_TRY(pd.alloc(Nsp * sizeof(double)));
+        SB_TRY(assemble_diag(c, clip_rows(dp, rc.lo, rc.hi), pd.d(), Nsp));
+        launch_sub(pd.d(), pd.d(), acc.d(), Ns, c->stream);
+        if (shard) {
+            if (Ns > 0) SB_CUDA(cudaMemcpyAsync(g_send_v, pd.p, Ns * sizeof(double), cudaMemcpyDeviceToDevice, c->stream));
         } else {
-            // cov = prior_full - V^T V  = prior_full - W W^T   (W now holds V^T, Nsp x Np)
-            DevBuf Cm(c);
-            SB_TRY(Cm.alloc((size_t)Nsp * Nsp * sizeof(double)));
-            SB_CUDA(cudaMemsetAsync(Cm.p, 0, (size_t)Nsp * Nsp * sizeof(double), c->stream));
-            SB_TRY(assemble_dense(c, dp, Cm.d(), Nsp));
-            launch_gemm_nt(W.d(), Nsp, W.d(), Nsp, Cm.d(), Nsp, Nsp, Nsp, Np, -1.0, 1.0, c->stream);
-            if (cov_out)
-                SB_CUDA(cudaMemcpy2DAsync(cov_out, Ns * sizeof(double), Cm.p, Nsp * sizeof(double),
-                                          Ns * sizeof(double), Ns, cudaMemcpyDefault, c->stream));
-            if (fac_out) {
-                // posterior covariance (+ noise) -> packed layout -> Cholesky, all on device.  append: the
-                // matrix factorised is the Schur complement S of the old head (see factor_splice), whose first
-                // r rows are the old rows of f's partial last block; otherwise r = 0 and S = Cm + noise.
-                const int64_t h = append ? f->N / NB * NB : 0;
-                const int r = (int)(append ? f->N - h : 0);
-                DevBuf nd(c);
-                const bool pn_dense = post_noise && post_noise->dense, pn_diag = post_noise && post_noise->diag;
-                if (pn_dense || pn_diag) {
-                    const size_t n = pn_dense ? (size_t)Ns * Ns : (size_t)Ns;
-                    SB_TRY(nd.alloc(n * sizeof(double)));
-                    SB_CUDA(cudaMemcpyAsync(nd.p, pn_dense ? post_noise->dense : post_noise->diag, n * sizeof(double),
-                                            cudaMemcpyDefault, c->stream));
-                }
-                launch_add_noise_dense(Cm.d(), Nsp, Ns, post_noise ? post_noise->sigma2 : 0.0, pn_diag && !pn_dense ? nd.d() : nullptr,
-                                       pn_dense ? nd.d() : nullptr, c->stream);
-                std::unique_ptr<sb_factor> fn;
-                SB_TRY(factor_alloc(c, r + Ns, fn));
-                launch_pack_schur(fn->L, r + Ns, r, Cm.d(), Nsp, r ? f->L.blk(h / NB, h / NB) : nullptr, f->L.ld(h / NB),
-                                  r ? W.d() + h * Nsp : nullptr, Nsp, c->stream);
-                launch_fill_padding(fn->L, r + Ns, c->stream);
-                int64_t info_s = 0;
-                const int32_t st = factor_finish(c, fn.get(), &info_s, /*force_local=*/true);
-                if (st == SB_ERR_NOT_POSDEF) {   // S's pivot index, in the order of the joint matrix
-                    if (info) *info = h + info_s;
-                    if (h > 0)
-                        sb::set_error("matrix is not positive definite; Cholesky factorization failed at pivot " +
-                                      std::to_string(h + info_s));
-                }
-                SB_TRY(st);
-                if (h > 0) {
-                    std::unique_ptr<sb_factor> joint;
-                    SB_TRY(factor_splice(c, f, fn.get(), W.d(), Nsp, Ns, joint));
-                    fn = std::move(joint);
-                }
-                *fac_out = fn.release();
-            }
-            SB_CUDA(cudaStreamSynchronize(c->stream));
+            SB_CUDA(cudaMemcpyAsync(var_out, pd.p, Ns * sizeof(double), cudaMemcpyDefault, c->stream));
         }
     }
     SB_CUDA(cudaGetLastError());
@@ -898,34 +940,37 @@ static int32_t predict_impl(sb_ctx* c, sb_factor* f, const sb_covspec* cross,
             SB_CUDA(cudaMemcpyAsync(var_out, g_recv_v, Ns_all * sizeof(double), cudaMemcpyDefault, c->stream));
         }
     }
-    cudaEventRecord(t1, c->stream);
-    SB_CUDA(cudaStreamSynchronize(c->stream));
-    float ms = 0;
-    cudaEventElapsedTime(&ms, t0, t1);
-    c->tm.predict_ms += ms;
-    c->tm.total_ms += ms;
-    count_launches(c, before);
-    return SB_OK;
-}
-
-int32_t sb_predict(sb_ctx* c, sb_factor* f, const sb_covspec* cross, const sb_covspec* prior_diag,
-                   void* mean_out, void* var_out) {
-    SB_CHECK(c && f && cross, "null argument");
-    return predict_impl(c, f, cross, prior_diag, false, mean_out, var_out, nullptr);
+    return call.end();
 }
 
 int32_t sb_predict_cov(sb_ctx* c, sb_factor* f, const sb_covspec* cross,
                        const sb_covspec* prior_full, void* cov_out) {
     SB_CHECK(c && f && cross && prior_full && cov_out, "null argument");
-    return predict_impl(c, f, cross, prior_full, true, nullptr, nullptr, cov_out);
+    SB_CHECK(cross->ncols == f->N, "cross spec must be N* x N");
+    Call call(c, Timed::predict);
+    const int64_t Ns = cross->nrows;
+    if (Ns == 0) return SB_OK;
+    PosteriorCov pc(c);
+    SB_TRY(pc.build(c, f, cross, prior_full));
+    SB_CUDA(cudaMemcpy2DAsync(cov_out, Ns * sizeof(double), pc.Cm.p, pc.x.rows_p * sizeof(double),
+                              Ns * sizeof(double), Ns, cudaMemcpyDefault, c->stream));
+    SB_CUDA(cudaStreamSynchronize(c->stream));
+    return call.end();
 }
 
+// cholesky(cov(f_post(x*)) + noise), formed and factorised on the device
 int32_t sb_predict_factor(sb_ctx* c, sb_factor* f, const sb_covspec* cross, const sb_covspec* prior_full,
                           const sb_noise* noise, sb_factor** out, int64_t* info) {
     SB_CHECK(c && f && cross && prior_full && out, "null argument");
     *out = nullptr;
     if (info) *info = 0;
-    return predict_impl(c, f, cross, prior_full, true, nullptr, nullptr, nullptr, noise, out, info);
+    SB_CHECK(cross->ncols == f->N, "cross spec must be N* x N");
+    Call call(c, Timed::predict);
+    if (cross->nrows == 0) return SB_OK;
+    PosteriorCov pc(c);
+    SB_TRY(pc.build(c, f, cross, prior_full));
+    SB_TRY(factor_posterior(c, f, pc, noise, 0, 0, out, info));
+    return call.end();
 }
 
 // Sequential conditioning without refactorising (AbstractGPs update_chol): the sweep V = K21 L^{-T} and
@@ -937,7 +982,13 @@ int32_t sb_factor_append(sb_ctx* c, sb_factor* f, const sb_covspec* cross, const
     *out = nullptr;
     if (info) *info = 0;
     SB_CHECK(cross->nrows > 0, "sb_factor_append: no new observations");
-    return predict_impl(c, f, cross, prior_full, true, nullptr, nullptr, nullptr, noise, out, info, /*append=*/true);
+    SB_CHECK(cross->ncols == f->N, "cross spec must be N* x N");
+    Call call(c, Timed::predict);
+    PosteriorCov pc(c);
+    SB_TRY(pc.build(c, f, cross, prior_full));
+    const int64_t h = f->N / NB * NB;
+    SB_TRY(factor_posterior(c, f, pc, noise, h, (int)(f->N - h), out, info));
+    return call.end();
 }
 
 // ---- gradients of logpdf (SURVEY 8f.1) ------------------------------------------------------------
@@ -945,10 +996,6 @@ int32_t sb_factor_append(sb_ctx* c, sb_factor* f, const sb_covspec* cross, const
 // src/affine_transformations/cross.jl:8-22 deliver in the reference (examples/getting_started/
 // script.jl:154-213).  K^{-1} = L^{-T} L^{-1} is formed once with the tensor-core sweep (I L^{-T}, then
 // one NT product), after which every term costs one fused O(N^2) reduction.
-static __global__ void set_identity_kernel(double* W, int64_t n) {
-    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) W[i * n + i] = 1.0;
-}
 static __global__ void qdiag_kernel(const double* alpha, const double* Kinv, int64_t ld, int64_t n, double* out) {
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) out[i] = 0.5 * (alpha[i] * alpha[i] - Kinv[i * ld + i]);
@@ -958,43 +1005,39 @@ int32_t sb_logpdf_grad(sb_ctx* c, sb_factor* f, const sb_covspec* spec, double* 
     SB_CHECK(c && f && spec && g_terms && g_noise_diag, "null argument");
     SB_CHECK(f->has_alpha, "sb_logpdf_grad needs alpha: call sb_factor_set_data(delta) first");
     SB_CHECK(spec->symmetric == 1 && spec->nrows == f->N && spec->ncols == f->N, "spec must be the symmetric N x N spec of the factor");
-    begin_call(c);
-    int64_t before = g_launch_count;
+    Call call(c);
     const int64_t N = f->N, Np = f->Np;
     DevSpec ds(c);
     SB_TRY(ds.build(spec, c->stream, false));
-    DevBuf W(c), Kinv(c), Xk(c), g(c), qd(c);
+    DevBuf W(c), Kinv(c), g(c), qd(c);
+    SweepWs ws(c);
     SB_TRY(W.alloc((size_t)Np * Np * sizeof(double)));
     SB_TRY(Kinv.alloc((size_t)Np * Np * sizeof(double)));
-    SB_TRY(Xk.alloc((size_t)Np * SWEEP_COLS * sizeof(double)));
+    SB_TRY(ws.init(Np, f->oz));
     SB_TRY(g.alloc((size_t)2 * (spec->nterms > 0 ? spec->nterms : 1) * sizeof(double)));
     SB_TRY(qd.alloc((size_t)N * sizeof(double)));
     SB_CUDA(cudaMemsetAsync(W.p, 0, (size_t)Np * Np * sizeof(double), c->stream));
     SB_CUDA(cudaMemsetAsync(g.p, 0, (size_t)2 * (spec->nterms > 0 ? spec->nterms : 1) * sizeof(double), c->stream));
-    set_identity_kernel<<<(unsigned)((Np + 255) / 256), 256, 0, c->stream>>>(W.d(), Np);
-    OzSweepWs ws(c);
-    if (f->oz) SB_TRY(ws.init(Np));
-    SB_TRY(trsm_sweep(c, f, W.d(), Np, Xk.d(), /*keep=*/true, nullptr, &ws));              // W = L^{-T}
+    launch_set_scaled_identity(W.d(), Np, 1.0, c->stream);
+    SB_TRY(trsm_sweep(c, f, W.d(), Np, ws, /*keep=*/true, nullptr));                       // W = L^{-T}
     launch_gemm_nt(W.d(), Np, W.d(), Np, Kinv.d(), Np, Np, Np, Np, 1.0, 0.0, c->stream);  // K^{-1} = W W'
     for (auto& b : ds.blocks) {
         const bool offdiag = b.row0 != b.col0;   // symmetric spec: blocks (i, j), j <= i; (i, i) is the full square
         launch_grad_reduce(b, f->alpha, Kinv.d(), Np, offdiag ? 2.0 : 1.0, g.d(), c->stream);
     }
     qdiag_kernel<<<(unsigned)((N + 255) / 256), 256, 0, c->stream>>>(f->alpha, Kinv.d(), Np, N, qd.d());
-    g_launch_count += 2;
+    g_launch_count++;
     SB_CUDA(cudaGetLastError());
     if (spec->nterms > 0)
         SB_CUDA(cudaMemcpyAsync(g_terms, g.p, (size_t)2 * spec->nterms * sizeof(double), cudaMemcpyDefault, c->stream));
     SB_CUDA(cudaMemcpyAsync(g_noise_diag, qd.p, (size_t)N * sizeof(double), cudaMemcpyDefault, c->stream));
     SB_CUDA(cudaStreamSynchronize(c->stream));
-    count_launches(c, before);
-    return SB_OK;
+    return call.end();
 }
 
 int32_t sb_rand(sb_ctx* c, sb_factor* f, const void* z, int32_t S, void* out) {
     SB_CHECK(c && f && z && out && S >= 1, "bad argument");
-    begin_call(c);
-    int64_t before = g_launch_count;
+    Call call(c);
     DevBuf zb(c), ob(c);
     SB_TRY(zb.alloc((size_t)f->Np * S * sizeof(double)));
     SB_TRY(ob.alloc((size_t)f->Np * S * sizeof(double)));
@@ -1004,8 +1047,7 @@ int32_t sb_rand(sb_ctx* c, sb_factor* f, const void* z, int32_t S, void* out) {
     SB_CUDA(cudaMemcpy2DAsync(out, f->N * sizeof(double), ob.p, f->Np * sizeof(double), f->N * sizeof(double),
                               S, cudaMemcpyDefault, c->stream));
     SB_CUDA(cudaStreamSynchronize(c->stream));
-    count_launches(c, before);
-    return SB_OK;
+    return call.end();
 }
 
 int32_t sb_factor_get_L(sb_ctx* c, sb_factor* f, void* L_out) {
@@ -1036,6 +1078,18 @@ struct sb_vfe {
 
 constexpr int64_t VFE_CHUNK_ROWS = 16384;  // observation rows per chunk of the K_fu stream
 
+// s2 = sigma_i^2 of the VFE observation noise (diagonal or scalar) read to the host and checked positive, and
+// sinv = sigma_i^{-1}
+static int32_t vfe_noise(const sb_noise* noise, int64_t N, double* s2, double* sinv) {
+    if (noise->diag) SB_CUDA(cudaMemcpy(s2, noise->diag, N * sizeof(double), cudaMemcpyDefault));
+    else for (int64_t i = 0; i < N; i++) s2[i] = noise->sigma2;
+    for (int64_t i = 0; i < N; i++) {
+        SB_CHECK(s2[i] > 0.0, "VFE needs positive observation noise");
+        sinv[i] = 1.0 / sqrt(s2[i]);
+    }
+    return SB_OK;
+}
+
 int32_t sb_vfe_destroy(sb_vfe* v) {
     if (!v) return SB_OK;
     cudaSetDevice(v->ctx->device);
@@ -1052,8 +1106,7 @@ int32_t sb_vfe_create(sb_ctx* c, const sb_covspec* uu, const sb_noise* noise_u, 
                       const sb_covspec* ff_diag, const sb_noise* noise_f, const void* delta, sb_vfe** out,
                       double* out2, int64_t* info) {
     SB_CHECK(c && uu && xu && ff_diag && noise_f && delta && out && out2, "null argument");
-    begin_call(c);
-    int64_t before = g_launch_count;
+    Call call(c, Timed::total);
     *out = nullptr;
     if (info) *info = 0;
     const int64_t N = xu->nrows, M = xu->ncols;
@@ -1064,8 +1117,6 @@ int32_t sb_vfe_create(sb_ctx* c, const sb_covspec* uu, const sb_noise* noise_u, 
 
     std::unique_ptr<sb_vfe> v(new sb_vfe(c));
     SB_TRY(factor_create_impl(c, uu, noise_u, v->fu, info, /*force_local=*/true));
-    cudaEvent_t t0 = c->next_event(), t1 = c->next_event();
-    cudaEventRecord(t0, c->stream);
     v->N = N;
     v->M = M;
     v->Mp = v->fu->Np;
@@ -1074,15 +1125,9 @@ int32_t sb_vfe_create(sb_ctx* c, const sb_covspec* uu, const sb_noise* noise_u, 
     // host O(N) prep: sigma^{-1}, delta~ = delta / sigma, log det Sigma_y, |delta~|^2
     std::vector<double> hd(N), sinv(N), hnoise(N);
     SB_CUDA(cudaMemcpy(hd.data(), delta, N * sizeof(double), cudaMemcpyDefault));
-    if (noise_f->diag) {
-        SB_CUDA(cudaMemcpy(hnoise.data(), noise_f->diag, N * sizeof(double), cudaMemcpyDefault));
-    } else {
-        for (int64_t i = 0; i < N; i++) hnoise[i] = noise_f->sigma2;
-    }
+    SB_TRY(vfe_noise(noise_f, N, hnoise.data(), sinv.data()));
     double logdet_sy = 0.0, dd = 0.0;
     for (int64_t i = 0; i < N; i++) {
-        SB_CHECK(hnoise[i] > 0.0, "VFE needs positive observation noise");
-        sinv[i] = 1.0 / sqrt(hnoise[i]);
         logdet_sy += log(hnoise[i]);
         hd[i] *= sinv[i];
         dd += hd[i] * hd[i];
@@ -1091,16 +1136,16 @@ int32_t sb_vfe_create(sb_ctx* c, const sb_covspec* uu, const sb_noise* noise_u, 
     DevSpec dxu(c), dff(c);
     SB_TRY(dxu.build(xu, c->stream, false));
     SB_TRY(dff.build(ff_diag, c->stream, true));
-    const std::vector<BlockDev> all_blocks = dxu.blocks;
 
     const int64_t NC = VFE_CHUNK_ROWS;
-    DevBuf dsinv(c), ddt(c), W(c), T(c), Xk(c), D(c), vv(c), fro(c), varf(c);
+    DevBuf dsinv(c), ddt(c), W(c), T(c), D(c), vv(c), fro(c), varf(c);
+    SweepWs ws(c);
     const int64_t nchunks_total = (N + NC - 1) / NC;
     SB_TRY(dsinv.alloc(N * sizeof(double)));
     SB_TRY(ddt.alloc(round_up(N, NC) * sizeof(double)));
     SB_TRY(W.alloc((size_t)NC * Mp * sizeof(double)));
     SB_TRY(T.alloc((size_t)NC * Mp * sizeof(double)));
-    SB_TRY(Xk.alloc((size_t)NC * SWEEP_COLS * sizeof(double)));
+    SB_TRY(ws.init(NC, v->fu->oz));
     SB_TRY(D.alloc((size_t)Mp * Mp * sizeof(double)));
     SB_TRY(vv.alloc((size_t)(Mp + 8) * sizeof(double)));
     SB_TRY(fro.alloc((size_t)(nchunks_total + 1) * sizeof(double)));
@@ -1112,18 +1157,12 @@ int32_t sb_vfe_create(sb_ctx* c, const sb_covspec* uu, const sb_noise* noise_u, 
     SB_CUDA(cudaMemsetAsync(vv.p, 0, (size_t)(Mp + 8) * sizeof(double), c->stream));
     SB_CUDA(cudaMemsetAsync(fro.p, 0, (size_t)(nchunks_total + 1) * sizeof(double), c->stream));
 
-    OzSweepWs ws(c);
-    if (v->fu->oz) SB_TRY(ws.init(NC));
     for (int64_t ci = c->rank; ci < nchunks_total; ci += c->world) {  // chunks round-robin over ranks
         const int64_t r0 = ci * NC, r1 = r0 + NC < N ? r0 + NC : N;
         const int64_t rows = r1 - r0, rows_p = round_up(rows, NB);
-        dxu.blocks = all_blocks;
-        dxu.nrows = N;
-        clip_rows(dxu, r0, r1, false);
-        SB_CUDA(cudaMemsetAsync(W.p, 0, (size_t)rows_p * Mp * sizeof(double), c->stream));
-        SB_TRY(assemble_dense(c, dxu, W.d(), rows_p));
+        SB_TRY(assemble_dense(c, clip_rows(dxu, r0, r1), W.d(), rows_p, Mp));
         launch_rowscale(W.d(), rows_p, rows, Mp, dsinv.d() + r0, c->stream);
-        SB_TRY(trsm_sweep(c, v->fu.get(), W.d(), rows_p, Xk.d(), /*keep=*/true, nullptr, &ws));
+        SB_TRY(trsm_sweep(c, v->fu.get(), W.d(), rows_p, ws, /*keep=*/true, nullptr));
         launch_colsumsq(W.d(), rows_p * Mp, 0, 1, fro.d() + ci, c->stream);
         launch_gemv_t(W.d(), rows_p, rows, Mp, ddt.d() + r0, vv.d(), c->stream);
         launch_transpose(W.d(), rows_p, rows_p, Mp, T.d(), Mp, c->stream);
@@ -1147,8 +1186,7 @@ int32_t sb_vfe_create(sb_ctx* c, const sb_covspec* uu, const sb_noise* noise_u, 
     tri_solve(c, v->fl.get(), vv.d(), 1, false);
     launch_colsumsq(vv.d(), Mp, Mp, 1, q.d(), c->stream);
     // var(f, x) for the trace term
-    SB_CUDA(cudaMemsetAsync(varf.p, 0, N * sizeof(double), c->stream));
-    SB_TRY(assemble_diag(c, dff, varf.d()));
+    SB_TRY(assemble_diag(c, dff.blocks, varf.d(), N));
     std::vector<double> hvar(N), hfro(nchunks_total);
     double hq = 0.0;
     SB_CUDA(cudaMemcpyAsync(hvar.data(), varf.p, N * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
@@ -1160,7 +1198,6 @@ int32_t sb_vfe_create(sb_ctx* c, const sb_covspec* uu, const sb_noise* noise_u, 
     SB_TRY(v->alpha.alloc((size_t)Mp * sizeof(double)));
     SB_CUDA(cudaMemcpyAsync(v->alpha, vv.p, v->alpha.bytes, cudaMemcpyDeviceToDevice, c->stream));
     SB_CUDA(cudaGetLastError());
-    cudaEventRecord(t1, c->stream);
     SB_CUDA(cudaStreamSynchronize(c->stream));
     double tr = 0.0, fro_sum = 0.0;
     for (int64_t i = 0; i < N; i++) tr += hvar[i] / hnoise[i];
@@ -1169,10 +1206,7 @@ int32_t sb_vfe_create(sb_ctx* c, const sb_covspec* uu, const sb_noise* noise_u, 
     const double dtc = -((double)N * log2pi + logdet_sy + v->fl->logdet + dd - hq) / 2.0;
     out2[0] = dtc - (tr - fro_sum) / 2.0;  // elbo
     out2[1] = dtc;
-    float ms = 0;
-    cudaEventElapsedTime(&ms, t0, t1);
-    c->tm.total_ms += ms;
-    count_launches(c, before);
+    SB_TRY(call.end());
     *out = v.release();
     return SB_OK;
 }
@@ -1197,34 +1231,26 @@ int32_t sb_vfe_grad(sb_ctx* c, sb_vfe* v, const sb_covspec* uu, const sb_covspec
     SB_CHECK(uu->nrows == M && uu->ncols == M && uu->symmetric == 1, "uu must be the symmetric M x M spec of cov(fz)");
     SB_CHECK(ff_diag->nrows == N && ff_diag->ncols == N, "ff_diag must be the N x N diag spec of var(f, x)");
     SB_CHECK(noise_f->dense == nullptr, "VFE needs diagonal observation noise");
-    begin_call(c);
-    int64_t before = g_launch_count;
-    cudaEvent_t t0 = c->next_event(), t1 = c->next_event();
-    cudaEventRecord(t0, c->stream);
+    Call call(c, Timed::total);
 
     // host O(N) prep: [delta | sigma^2 | sigma^-1 | d elbo / d K_ff[i,i]]
     std::vector<double> hobs(4 * N);
     double* hd = hobs.data();
     double* hs2 = hd + N;
     SB_CUDA(cudaMemcpy(hd, delta, N * sizeof(double), cudaMemcpyDefault));
-    if (noise_f->diag) SB_CUDA(cudaMemcpy(hs2, noise_f->diag, N * sizeof(double), cudaMemcpyDefault));
-    else for (int64_t i = 0; i < N; i++) hs2[i] = noise_f->sigma2;
-    for (int64_t i = 0; i < N; i++) {
-        SB_CHECK(hs2[i] > 0.0, "VFE needs positive observation noise");
-        hd[2 * N + i] = 1.0 / sqrt(hs2[i]);
-        hd[3 * N + i] = -0.5 / hs2[i];
-    }
+    SB_TRY(vfe_noise(noise_f, N, hs2, hd + 2 * N));
+    for (int64_t i = 0; i < N; i++) hd[3 * N + i] = -0.5 / hs2[i];
 
     DevSpec duu(c), dxu(c), dff(c);
     SB_TRY(duu.build(uu, c->stream, false));
     SB_TRY(dxu.build(xu, c->stream, false));
     SB_TRY(dff.build(ff_diag, c->stream, true));
-    const std::vector<BlockDev> xu_blocks = dxu.blocks, ff_blocks = dff.blocks;
     const int64_t NC = VFE_CHUNK_ROWS < round_up(N, NB) ? VFE_CHUNK_ROWS : round_up(N, NB);
     const int64_t nchunks_total = (N + VFE_CHUNK_ROWS - 1) / VFE_CHUNK_ROWS;
     const int64_t nuu = 2 * (int64_t)uu->nterms, nxu = 2 * (int64_t)xu->nterms, nff = 2 * (int64_t)ff_diag->nterms;
     const size_t mm = (size_t)Mp * Mp;
-    DevBuf obs(c), part(c), guu(c), gnu(c), Wu(c), Et(c), A1(c), A2(c), W(c), S(c), Xk(c), cv(c);
+    DevBuf obs(c), part(c), guu(c), gnu(c), Wu(c), Et(c), A1(c), A2(c), W(c), S(c), cv(c);
+    SweepWs ws(c);
     SB_TRY(obs.alloc(4 * N * sizeof(double)));
     SB_TRY(part.alloc((nxu + nff + N) * sizeof(double)));   // chunk partial sums: [g_xu | g_ff | g_noise_f]
     SB_TRY(guu.alloc((nuu > 0 ? nuu : 1) * sizeof(double)));
@@ -1232,7 +1258,7 @@ int32_t sb_vfe_grad(sb_ctx* c, sb_vfe* v, const sb_covspec* uu, const sb_covspec
     for (DevBuf* b : {&Wu, &Et, &A1, &A2}) SB_TRY(b->alloc(mm * sizeof(double)));
     SB_TRY(W.alloc((size_t)NC * Mp * sizeof(double)));
     SB_TRY(S.alloc((size_t)NC * Mp * sizeof(double)));
-    SB_TRY(Xk.alloc((size_t)(NC > Mp ? NC : Mp) * SWEEP_COLS * sizeof(double)));
+    SB_TRY(ws.init(NC > Mp ? NC : Mp, /*int8=*/false));   // one X buffer for the prologue and the chunks
     SB_TRY(cv.alloc((size_t)5 * NC * sizeof(double)));
     const double* d_delta = obs.d();
     const double* d_s2 = obs.d() + N;
@@ -1250,13 +1276,14 @@ int32_t sb_vfe_grad(sb_ctx* c, sb_vfe* v, const sb_covspec* uu, const sb_covspec
     SB_CUDA(cudaMemsetAsync(part.p, 0, part.bytes, c->stream));
     SB_CUDA(cudaMemsetAsync(guu.p, 0, guu.bytes, c->stream));
 
-    // M^3 prologue (DMMA sweeps and products): E^T = L_u^{-T} (I - B^{-1}) and P = L_u^{-T} D E
+    // M^3 prologue (DMMA sweeps, as ws has no digit planes yet, and products): E^T = L_u^{-T} (I - B^{-1}) and
+    // P = L_u^{-T} D E
     for (DevBuf* b : {&Wu, &A1, &A2}) SB_CUDA(cudaMemsetAsync(b->p, 0, mm * sizeof(double), c->stream));
     launch_set_scaled_identity(Wu.d(), Mp, 1.0, c->stream);
     launch_set_scaled_identity(A1.d(), Mp, 1.0, c->stream);
     launch_set_scaled_identity(A2.d(), Mp, 1.0, c->stream);
-    SB_TRY(trsm_sweep(c, v->fu.get(), Wu.d(), Mp, Xk.d(), /*keep=*/true, nullptr));         // Wu = L_u^{-T}
-    SB_TRY(trsm_sweep(c, v->fl.get(), A1.d(), Mp, Xk.d(), /*keep=*/true, nullptr));         // A1 = L_B^{-T}
+    SB_TRY(trsm_sweep(c, v->fu.get(), Wu.d(), Mp, ws, /*keep=*/true, nullptr));            // Wu = L_u^{-T}
+    SB_TRY(trsm_sweep(c, v->fl.get(), A1.d(), Mp, ws, /*keep=*/true, nullptr));            // A1 = L_B^{-T}
     launch_gemm_nt(A1.d(), Mp, A1.d(), Mp, A2.d(), Mp, Mp, Mp, Mp, -1.0, 1.0, c->stream);  // A2 = I - B^{-1}
     launch_gemm_nt(Wu.d(), Mp, A2.d(), Mp, Et.d(), Mp, Mp, Mp, Mp, 1.0, 0.0, c->stream);   // E^T
     launch_unpack_lower(v->fl->L, Mp, A1.d(), c->stream);                                  // A1 = L_B
@@ -1273,32 +1300,24 @@ int32_t sb_vfe_grad(sb_ctx* c, sb_vfe* v, const sb_covspec* uu, const sb_covspec
     SB_CUDA(cudaGetLastError());
 
     // the observation stream: the chunks of sb_vfe_create, round-robin over ranks
-    OzSweepWs ws(c);
-    if (v->fu->oz || v->fl->oz) SB_TRY(ws.init(NC));
+    if (v->fu->oz || v->fl->oz) SB_TRY(ws.add_planes(NC));
     for (int64_t ci = c->rank; ci < nchunks_total; ci += c->world) {
         const int64_t r0 = ci * VFE_CHUNK_ROWS, r1 = r0 + VFE_CHUNK_ROWS < N ? r0 + VFE_CHUNK_ROWS : N;
         const int64_t rows = r1 - r0, rows_p = round_up(rows, NB);
-        dxu.blocks = xu_blocks;
-        dxu.nrows = N;
-        clip_rows(dxu, r0, r1, false);
-        dff.blocks = ff_blocks;
-        dff.nrows = dff.ncols = N;
-        clip_rows(dff, r0, r1, true);
-        SB_CUDA(cudaMemsetAsync(W.p, 0, (size_t)rows_p * Mp * sizeof(double), c->stream));
+        const std::vector<BlockDev> xu_rows = clip_rows(dxu, r0, r1), ff_rows = clip_rows(dff, r0, r1);
         SB_CUDA(cudaMemsetAsync(la, 0, 2 * NC * sizeof(double), c->stream));   // la, lb
-        SB_CUDA(cudaMemsetAsync(kff, 0, NC * sizeof(double), c->stream));
-        SB_TRY(assemble_dense(c, dxu, W.d(), rows_p));                                        // K_fu rows
+        SB_TRY(assemble_dense(c, xu_rows, W.d(), rows_p, Mp));                              // K_fu rows
         launch_gemv_n(W.d(), rows_p, rows_p, Mp, v->alpha, t, c->stream);                    // t = K_fu alpha
         launch_vfe_beta(d_delta + r0, t, d_s2 + r0, rows, rows_p, beta, c->stream);
         launch_rowscale(W.d(), rows_p, rows, Mp, d_sinv + r0, c->stream);
-        SB_TRY(trsm_sweep(c, v->fu.get(), W.d(), rows_p, Xk.d(), /*keep=*/true, la, &ws));  // A' rows, |a_i|^2
+        SB_TRY(trsm_sweep(c, v->fu.get(), W.d(), rows_p, ws, /*keep=*/true, la));           // A' rows, |a_i|^2
         launch_gemm_nt(W.d(), rows_p, Et.d(), Mp, S.d(), rows_p, rows_p, Mp, Mp, 1.0, 0.0, c->stream);
         launch_rowscale(S.d(), rows_p, rows, Mp, d_sinv + r0, c->stream);                    // S = Sigma^{-1/2} A' E
-        for (auto& b : dxu.blocks)
+        for (auto& b : xu_rows)
             launch_grad_reduce_outer(b, 1.0, beta, v->alpha, 1.0, S.d(), rows_p, 1.0, g_part_xu, c->stream);
-        SB_TRY(assemble_diag(c, dff, kff));
-        for (auto& b : dff.blocks) launch_grad_diag(b, d_wff + r0, g_part_ff, c->stream);
-        SB_TRY(trsm_sweep(c, v->fl.get(), W.d(), rows_p, Xk.d(), /*keep=*/false, lb, &ws)); // |L_B^{-1} a_i|^2
+        SB_TRY(assemble_diag(c, ff_rows, kff, NC));
+        for (auto& b : ff_rows) launch_grad_diag(b, d_wff + r0, g_part_ff, c->stream);
+        SB_TRY(trsm_sweep(c, v->fl.get(), W.d(), rows_p, ws, /*keep=*/false, lb));          // |L_B^{-1} a_i|^2
         launch_vfe_noise_grad(beta, la, lb, kff, d_s2 + r0, rows, g_part_nf + r0, c->stream);
     }
     SB_CUDA(cudaGetLastError());
@@ -1309,13 +1328,8 @@ int32_t sb_vfe_grad(sb_ctx* c, sb_vfe* v, const sb_covspec* uu, const sb_covspec
     if (nff > 0) SB_CUDA(cudaMemcpyAsync(g_ff, g_part_ff, nff * sizeof(double), cudaMemcpyDefault, c->stream));
     SB_CUDA(cudaMemcpyAsync(g_noise_u_diag, gnu.p, M * sizeof(double), cudaMemcpyDefault, c->stream));
     SB_CUDA(cudaMemcpyAsync(g_noise_f_diag, g_part_nf, N * sizeof(double), cudaMemcpyDefault, c->stream));
-    cudaEventRecord(t1, c->stream);
     SB_CUDA(cudaStreamSynchronize(c->stream));
-    float ms = 0;
-    cudaEventElapsedTime(&ms, t0, t1);
-    c->tm.total_ms += ms;
-    count_launches(c, before);
-    return SB_OK;
+    return call.end();
 }
 
 // cov(f_approx_post(x*)) = K** - B'B + (L_Lambda^{-1} B)'(L_Lambda^{-1} B),  B = L_u^{-1} K_u*
@@ -1325,78 +1339,68 @@ int32_t sb_vfe_predict_cov(sb_ctx* c, sb_vfe* v, const sb_covspec* cross, const 
     SB_CHECK(c && v && cross && prior_full && cov_out, "null argument");
     SB_CHECK(cross->ncols == v->M, "cross spec must be N* x M");
     SB_CHECK(prior_full->nrows == cross->nrows && prior_full->ncols == cross->nrows, "prior spec must be N* x N*");
-    begin_call(c);
-    int64_t before = g_launch_count;
-    const int64_t Ns = cross->nrows, Nsp = round_up(Ns > 0 ? Ns : 1, NB), Mp = v->Mp;
+    Call call(c);
+    const int64_t Ns = cross->nrows, Mp = v->Mp;
     if (Ns == 0) return SB_OK;
     DevSpec dc(c), dp(c);
     SB_TRY(dc.build(cross, c->stream, false));
     SB_TRY(dp.build(prior_full, c->stream, false));
-    DevBuf W(c), Xk(c), Cm(c);
-    SB_TRY(W.alloc((size_t)Nsp * Mp * sizeof(double)));
-    SB_TRY(Xk.alloc((size_t)Nsp * SWEEP_COLS * sizeof(double)));
+    CrossRows x(c);
+    SB_TRY(x.assemble(dc, 0, Ns, Mp));
+    const int64_t Nsp = x.rows_p;
+    DevBuf Cm(c);
     SB_TRY(Cm.alloc((size_t)Nsp * Nsp * sizeof(double)));
-    SB_CUDA(cudaMemsetAsync(W.p, 0, (size_t)Nsp * Mp * sizeof(double), c->stream));
-    SB_CUDA(cudaMemsetAsync(Cm.p, 0, (size_t)Nsp * Nsp * sizeof(double), c->stream));
-    SB_TRY(assemble_dense(c, dc, W.d(), Nsp));
-    SB_TRY(assemble_dense(c, dp, Cm.d(), Nsp));
-    OzSweepWs ws(c);
-    if (v->fu->oz || v->fl->oz) SB_TRY(ws.init(Nsp));
-    SB_TRY(trsm_sweep(c, v->fu.get(), W.d(), Nsp, Xk.d(), true, nullptr, &ws));      // W = B'
-    launch_gemm_nt(W.d(), Nsp, W.d(), Nsp, Cm.d(), Nsp, Nsp, Nsp, Mp, -1.0, 1.0, c->stream);
-    SB_TRY(trsm_sweep(c, v->fl.get(), W.d(), Nsp, Xk.d(), true, nullptr, &ws));      // W = (L_Lambda^{-1} B)'
-    launch_gemm_nt(W.d(), Nsp, W.d(), Nsp, Cm.d(), Nsp, Nsp, Nsp, Mp, 1.0, 1.0, c->stream);
+    SB_TRY(assemble_dense(c, dp.blocks, Cm.d(), Nsp, Nsp));
+    SB_TRY(x.ws.init(Nsp, v->fu->oz || v->fl->oz));
+    SB_TRY(x.sweep(v->fu.get(), true, nullptr));      // W = B'
+    launch_gemm_nt(x.W.d(), Nsp, x.W.d(), Nsp, Cm.d(), Nsp, Nsp, Nsp, Mp, -1.0, 1.0, c->stream);
+    SB_TRY(x.sweep(v->fl.get(), true, nullptr));      // W = (L_Lambda^{-1} B)'
+    launch_gemm_nt(x.W.d(), Nsp, x.W.d(), Nsp, Cm.d(), Nsp, Nsp, Nsp, Mp, 1.0, 1.0, c->stream);
     SB_CUDA(cudaGetLastError());
     SB_CUDA(cudaMemcpy2DAsync(cov_out, Ns * sizeof(double), Cm.p, Nsp * sizeof(double), Ns * sizeof(double), Ns,
                               cudaMemcpyDefault, c->stream));
     SB_CUDA(cudaStreamSynchronize(c->stream));
-    count_launches(c, before);
-    return SB_OK;
+    return call.end();
 }
 
 int32_t sb_vfe_predict(sb_ctx* c, sb_vfe* v, const sb_covspec* cross, const sb_covspec* prior_diag,
                        void* mean_out, void* var_out) {
     SB_CHECK(c && v && cross, "null argument");
     SB_CHECK(cross->ncols == v->M, "cross spec must be N* x M");
-    begin_call(c);
-    int64_t before = g_launch_count;
-    const int64_t Ns = cross->nrows, Nsp = round_up(Ns > 0 ? Ns : 1, NB), Mp = v->Mp;
+    Call call(c);
+    const int64_t Ns = cross->nrows, Mp = v->Mp;
     if (Ns == 0) return SB_OK;
     DevSpec dc(c), dp(c);
     SB_TRY(dc.build(cross, c->stream, false));
-    DevBuf W(c), Xk(c), mean(c), acc1(c), acc2(c), pd(c);
-    SB_TRY(W.alloc((size_t)Nsp * Mp * sizeof(double)));
-    SB_CUDA(cudaMemsetAsync(W.p, 0, (size_t)Nsp * Mp * sizeof(double), c->stream));
-    SB_TRY(assemble_dense(c, dc, W.d(), Nsp));
+    CrossRows x(c);
+    SB_TRY(x.assemble(dc, 0, Ns, Mp));
+    const int64_t Nsp = x.rows_p;
+    DevBuf mean(c), acc1(c), acc2(c), pd(c);
     if (mean_out) {
         SB_TRY(mean.alloc(Nsp * sizeof(double)));
-        launch_gemv_n(W.d(), Nsp, Nsp, Mp, v->alpha, mean.d(), c->stream);
+        launch_gemv_n(x.W.d(), Nsp, Nsp, Mp, v->alpha, mean.d(), c->stream);
         SB_CUDA(cudaMemcpyAsync(mean_out, mean.p, Ns * sizeof(double), cudaMemcpyDefault, c->stream));
     }
     if (var_out) {
         SB_CHECK(prior_diag && prior_diag->nrows == Ns, "prior diag spec required for var");
         SB_TRY(dp.build(prior_diag, c->stream, true));
-        SB_TRY(Xk.alloc((size_t)Nsp * SWEEP_COLS * sizeof(double)));
         SB_TRY(acc1.alloc(Nsp * sizeof(double)));
         SB_TRY(acc2.alloc(Nsp * sizeof(double)));
         SB_TRY(pd.alloc(Nsp * sizeof(double)));
         SB_CUDA(cudaMemsetAsync(acc1.p, 0, Nsp * sizeof(double), c->stream));
         SB_CUDA(cudaMemsetAsync(acc2.p, 0, Nsp * sizeof(double), c->stream));
-        SB_CUDA(cudaMemsetAsync(pd.p, 0, Nsp * sizeof(double), c->stream));
         // B^T = K_*u L_u^{-T} (kept), then (L_Lambda^{-1} B)^T = B^T L_Lambda^{-T}
-        OzSweepWs ws(c);
-        if (v->fu->oz || v->fl->oz) SB_TRY(ws.init(Nsp));
-        SB_TRY(trsm_sweep(c, v->fu.get(), W.d(), Nsp, Xk.d(), true, acc1.d(), &ws));
-        SB_TRY(trsm_sweep(c, v->fl.get(), W.d(), Nsp, Xk.d(), false, acc2.d(), &ws));
-        SB_TRY(assemble_diag(c, dp, pd.d()));
+        SB_TRY(x.ws.init(Nsp, v->fu->oz || v->fl->oz));
+        SB_TRY(x.sweep(v->fu.get(), true, acc1.d()));
+        SB_TRY(x.sweep(v->fl.get(), false, acc2.d()));
+        SB_TRY(assemble_diag(c, dp.blocks, pd.d(), Nsp));
         launch_sub(pd.d(), pd.d(), acc1.d(), Ns, c->stream);    // k** - |B|^2
         launch_axpy1(pd.d(), acc2.d(), Ns, c->stream);          //     + |L_Lambda^{-1} B|^2
         SB_CUDA(cudaMemcpyAsync(var_out, pd.p, Ns * sizeof(double), cudaMemcpyDefault, c->stream));
     }
     SB_CUDA(cudaGetLastError());
     SB_CUDA(cudaStreamSynchronize(c->stream));
-    count_launches(c, before);
-    return SB_OK;
+    return call.end();
 }
 
 }  // extern "C"

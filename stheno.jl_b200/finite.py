@@ -103,9 +103,7 @@ class FiniteGP:
         self._lowered = None
         if isinstance(f, (GPPP, SthenoAbstractGP)):
             self.prior, self.post = f, None
-        elif isinstance(f, PosteriorGP):
-            self.prior, self.post = f.prior, f
-        elif isinstance(f, ApproxPosteriorGP):
+        elif isinstance(f, _Posterior):
             self.prior, self.post = f.prior, f
         else:
             raise TypeError(f"cannot index a {type(f).__name__}")
@@ -233,7 +231,7 @@ def mean(f, x=None):
         return mean(f.f, f.x)
     if isinstance(f, SparseFiniteGP):
         return mean(f.fobs)
-    if isinstance(f, (PosteriorGP, ApproxPosteriorGP)):
+    if isinstance(f, _Posterior):
         return f.mean(x)
     return _prior_mean(f, x)
 
@@ -252,7 +250,7 @@ def cov(f, x=None, y=None):
             return K + np.asarray(f.noise)
         K[np.diag_indices_from(K)] += f.noise_diag()
         return K
-    if isinstance(f, (PosteriorGP, ApproxPosteriorGP)):
+    if isinstance(f, _Posterior):
         return f.cov(x, y)
     lx = Lowered(f, x)
     ly = lx if y is None else Lowered(f, y)
@@ -266,7 +264,7 @@ def cov(f, x=None, y=None):
 def var(f, x=None, y=None):
     if isinstance(f, FiniteGP):
         return var(f.f, f.x) + f.noise_diag()
-    if isinstance(f, (PosteriorGP, ApproxPosteriorGP)):
+    if isinstance(f, _Posterior):
         return f.var(x)
     lx = Lowered(f, x)
     ly = None if y is None else Lowered(f, y)
@@ -283,7 +281,7 @@ def mean_and_var(f, x=None):
             m, v = f.post.mean_and_var(f.x)
             return m, v + f.noise_diag()
         return mean(f), var(f)
-    if isinstance(f, (PosteriorGP, ApproxPosteriorGP)):
+    if isinstance(f, _Posterior):
         return f.mean_and_var(x)
     return mean(f, x), var(f, x)
 
@@ -340,10 +338,63 @@ def rand(fx, z):
     return out[:, 0] + m if z.ndim == 1 else out + m[:, None]
 
 
-class PosteriorGP:
+class _Posterior:
+    """Predictions of a posterior process on the device.  A subclass supplies its ABI calls (`_PREDICT`: mean / var,
+    `_COV`: dense covariance), its device handle (`_handle`) and the lowered inputs of its training side (`_train`)."""
+
+    def __call__(self, x, noise=1e-18):
+        return FiniteGP(self, x, noise)
+
+    def _install_alpha(self):
+        """Make the device handle hold this posterior's weights before a mean is predicted from it."""
+
+    def _predict(self, x, want_mean, want_var):
+        ls = Lowered(self.prior, x)
+        cross = spec_dense(ls, self._train)
+        pd = spec_diag(ls) if want_var else None
+        m = np.empty(ls.n) if want_mean else None
+        v = np.empty(ls.n) if want_var else None
+        if want_mean:
+            self._install_alpha()
+        _lib.check(getattr(_lib.load(), self._PREDICT)(
+            self._handle.ctx.h, self._handle.h, C.byref(cross), C.byref(pd) if pd is not None else None,
+            m.ctypes.data if m is not None else None, v.ctypes.data if v is not None else None))
+        if m is not None:
+            m += ls.mean()
+        return m, v
+
+    def mean(self, x):
+        return self._predict(x, True, False)[0]
+
+    def var(self, x):
+        return self._predict(x, False, True)[1]
+
+    def mean_and_var(self, x):
+        return self._predict(x, True, True)
+
+    def cov(self, x, y=None):
+        """cov(f_post, x) and cov(f_post, x, z).  The cross form evaluates the joint posterior covariance of the
+        stacked inputs [x; z] on the device and returns its off-diagonal block."""
+        if y is not None:
+            nx = npoints(x)
+            K = self.cov(_stack_inputs(self.prior, x, y))
+            return np.asfortranarray(K[:nx, nx:])
+        ls = Lowered(self.prior, x)
+        cross = spec_dense(ls, self._train)
+        full = spec_dense(ls, ls)
+        K = np.empty((ls.n, ls.n), dtype=np.float64, order="F")
+        _lib.check(getattr(_lib.load(), self._COV)(self._handle.ctx.h, self._handle.h, C.byref(cross), C.byref(full),
+                                                   K.ctypes.data))
+        return K
+
+
+class PosteriorGP(_Posterior):
     """`posterior(fx, y)`: shares the device factor of `fx` and keeps ITS OWN alpha = C \\ (y - m)
     (AbstractGPs PosteriorGP stores (alpha, C, x, delta); `posterior` is a pure function, so two
-    posteriors built from one fx must not see each other's data)."""
+    posteriors built from one fx must not see each other's data).
+    cov(f_post, x, z) = K(x,z) - (C.U'\\K_{X,x})'(C.U'\\K_{X,z}) (AbstractGPs, SURVEY App. A)."""
+
+    _PREDICT, _COV = "sb_predict", "sb_predict_cov"
 
     def __init__(self, fx: FiniteGP, y):
         y = np.asarray(y, dtype=np.float64)
@@ -361,8 +412,13 @@ class PosteriorGP:
         _lib.check(lib.sb_factor_alpha(self.fac.ctx.h, self.fac.h, self._alpha.ctypes.data))
         self.fac.alpha_owner = self
 
-    def __call__(self, x, noise=1e-18):
-        return FiniteGP(self, x, noise)
+    @property
+    def _handle(self):
+        return self.fac
+
+    @property
+    def _train(self):
+        return self.lx
 
     @property
     def alpha(self):
@@ -372,46 +428,6 @@ class PosteriorGP:
         if self.fac.alpha_owner is not self:
             _lib.check(_lib.load().sb_factor_set_alpha(self.fac.ctx.h, self.fac.h, self._alpha.ctypes.data))
             self.fac.alpha_owner = self
-
-    def _predict(self, x, want_mean, want_var):
-        ls = Lowered(self.prior, x)
-        cross = spec_dense(ls, self.lx)
-        pd = spec_diag(ls) if want_var else None
-        m = np.empty(ls.n) if want_mean else None
-        v = np.empty(ls.n) if want_var else None
-        if want_mean:
-            self._install_alpha()
-        _lib.check(_lib.load().sb_predict(
-            self.fac.ctx.h, self.fac.h, C.byref(cross), C.byref(pd) if pd is not None else None,
-            m.ctypes.data if m is not None else None, v.ctypes.data if v is not None else None))
-        if m is not None:
-            m += ls.mean()
-        return m, v
-
-    def mean(self, x):
-        return self._predict(x, True, False)[0]
-
-    def var(self, x):
-        return self._predict(x, False, True)[1]
-
-    def mean_and_var(self, x):
-        return self._predict(x, True, True)
-
-    def cov(self, x, y=None):
-        """cov(f_post, x) and cov(f_post, x, z) = K(x,z) - (C.U'\\K_{X,x})'(C.U'\\K_{X,z})
-        (AbstractGPs, SURVEY App. A).  The cross form evaluates the joint posterior covariance of
-        the stacked inputs [x; z] on the device and returns its off-diagonal block."""
-        if y is not None:
-            nx = npoints(x)
-            K = self.cov(_stack_inputs(self.prior, x, y))
-            return np.asfortranarray(K[:nx, nx:])
-        ls = Lowered(self.prior, x)
-        cross = spec_dense(ls, self.lx)
-        full = spec_dense(ls, ls)
-        K = np.empty((ls.n, ls.n), dtype=np.float64, order="F")
-        _lib.check(_lib.load().sb_predict_cov(self.fac.ctx.h, self.fac.h, C.byref(cross), C.byref(full),
-                                              K.ctypes.data))
-        return K
 
 
 def _stack_inputs(prior, x, z):
@@ -580,50 +596,24 @@ def grad_elbo(v, fx=None, y=None) -> ElboGradient:
     return ElboGradient(e, noise, inducing, list(agg.values()))
 
 
-class ApproxPosteriorGP:
+class ApproxPosteriorGP(_Posterior):
+    """`posterior(VFE(fz), fx, y)`: the VFE handle holds its own weights.  cov(f_approx_post, x) =
+    K** - B'B + (Lambda.U'\\B)'(Lambda.U'\\B) with B = U' \\ K_{z*} (AbstractGPs approx posterior)."""
+
+    _PREDICT, _COV = "sb_vfe_predict", "sb_vfe_predict_cov"
+
     def __init__(self, v: VFE, fx: FiniteGP, y):
         self.prior = fx.prior
         self.lz = v.fz.lowered
         self.handle, self.elbo, self.dtc = _vfe_create(v, fx, y)
 
-    def __call__(self, x, noise=1e-18):
-        return FiniteGP(self, x, noise)
+    @property
+    def _handle(self):
+        return self.handle
 
-    def _predict(self, x, want_mean, want_var):
-        ls = Lowered(self.prior, x)
-        cross = spec_dense(ls, self.lz)
-        pd = spec_diag(ls) if want_var else None
-        m = np.empty(ls.n) if want_mean else None
-        vv = np.empty(ls.n) if want_var else None
-        _lib.check(_lib.load().sb_vfe_predict(
-            self.handle.ctx.h, self.handle.h, C.byref(cross), C.byref(pd) if pd is not None else None,
-            m.ctypes.data if m is not None else None, vv.ctypes.data if vv is not None else None))
-        if m is not None:
-            m += ls.mean()
-        return m, vv
-
-    def mean(self, x):
-        return self._predict(x, True, False)[0]
-
-    def var(self, x):
-        return self._predict(x, False, True)[1]
-
-    def mean_and_var(self, x):
-        return self._predict(x, True, True)
-
-    def cov(self, x, y=None):
-        """K** - B'B + (Lambda.U'\\B)'(Lambda.U'\\B) with B = U' \\ K_{z*} (AbstractGPs approx posterior)."""
-        if y is not None:
-            nx = npoints(x)
-            K = self.cov(_stack_inputs(self.prior, x, y))
-            return np.asfortranarray(K[:nx, nx:])
-        ls = Lowered(self.prior, x)
-        cross = spec_dense(ls, self.lz)
-        full = spec_dense(ls, ls)
-        K = np.empty((ls.n, ls.n), dtype=np.float64, order="F")
-        _lib.check(_lib.load().sb_vfe_predict_cov(self.handle.ctx.h, self.handle.h, C.byref(cross), C.byref(full),
-                                                  K.ctypes.data))
-        return K
+    @property
+    def _train(self):
+        return self.lz
 
 
 def approx_posterior(v: VFE, fx: FiniteGP, y):
